@@ -1,14 +1,16 @@
 #!/usr/bin/env python
-"""bench.py — CSNet forward throughput on B200 (BASELINE.json configs[1]: csnet-L-x2 inference, bs 256,
+"""bench.py — CSNet forward throughput on H100 (BASELINE.json configs[1]: csnet-L-x2 inference, bs 256,
 224x224, fp16 activation storage / fp32 accumulate), one process per GPU.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 Prints ONE JSON line (rank 0).  `value` = whole-job images/s with inputs resident in HBM; `e2e` = the same
 through the host-buffer C-ABI call (H2D + program + D2H per step, pinned memory); `roofline` = the dominant
 kernel's algorithmic bytes / its live CUDA-event time vs the measured HBM peak; `cpu_baseline` = the oracle
 port (same ATen calls the reference makes) timed on this box's host cores on a bounded sample.
-`--impl reference` times that CPU implementation as the reference arm.
+`--impl reference` times that CPU implementation as the reference arm.  `--dump-outputs DIR` writes what the timed path
+returned in its last step as DIR/<name>.npy (float32), so that two builds can be compared output for output on the same
+seeded inputs.
 """
 from __future__ import annotations
 
@@ -26,6 +28,7 @@ if ROOT not in sys.path:
 
 METRIC = "images/sec CSNet fwd 224x224"
 UNIT = "images/s"
+H100_HBM_GBS, H100_FP16_TFLOPS = 3350.0, 989.0      # H100 SXM data sheet (700 W): HBM3 bandwidth, dense fp16 tensor rate
 
 
 def parse():
@@ -49,14 +52,38 @@ def parse():
                     help="train sub-record with ILBlock-granular recompute (Trainer(recompute=True)): ~3x less activation memory, one extra forward")
     ap.add_argument("--no-extras", action="store_true",
                     help="skip the train sub-record, the eager-GPU baseline and the extra configs (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs to DIR/<name>.npy (float32, at most 64 MB in all)")
     return ap.parse_args()
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(d, arrays):
+    """Write each float array as d/<name>.npy in float32.  An array over the byte budget left is cut to a fixed, seeded
+    sample of its first-axis entries (sorted), whose indices go to d/<name>_index.npy."""
+    import numpy as np
+
+    os.makedirs(d, exist_ok=True)
+    left = DUMP_BYTES
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(np.asarray(a, dtype=np.float32))
+        if a.nbytes > left and a.ndim > 0 and a.shape[0] > 1:
+            per = a.nbytes // a.shape[0]
+            k = max(1, min(a.shape[0], left // max(per, 1)))
+            idx = np.sort(np.random.default_rng(0).choice(a.shape[0], size=k, replace=False))
+            np.save(os.path.join(d, f"{name}_index.npy"), idx.astype(np.int64))
+            a = a[idx]
+        np.save(os.path.join(d, f"{name}.npy"), a)
+        left -= a.nbytes
 
 
 def workload_config(a, world):
     return {"workload": f"{a.model} inference, {a.batch} img/GPU x {a.size}x{a.size}, {a.dtype} storage / fp32 accumulate",
             "model_weights": "shipped checkpoint (tests/golden npz)", "per_gpu_batch": a.batch,
             "global_batch": a.batch * world, "size": a.size, "parallelism": f"dp{world} (independent batches, no collective)",
-            "l2": "activations of one step (>2 GB) exceed the 126 MB L2; no explicit flush"}
+            "l2": "activations of one step (>2 GB) exceed the 50 MB L2; no explicit flush"}
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -74,7 +101,7 @@ def cpu_forward_timer(a, n_img):
 
     def step():
         with torch.no_grad():
-            O.csnet_forward(cfg, sd, x)
+            return O.csnet_forward(cfg, sd, x)
 
     # "all the host threads it can use": these are ~400 tiny ATen calls per forward, and oversubscribing a
     # 100+-thread box makes them SLOWER (measured 0.3 img/s at 128 threads vs 8.7 img/s at 8), so pick the
@@ -113,11 +140,13 @@ def run_reference(a, rank):
     step, cores = cpu_forward_timer(a, a.cpu_sample)
     for _ in range(max(1, min(a.warmup, 2))):
         step()
-    k = max(1, min(a.steps, 10))                     # bounded: each step is a few seconds of CPU work
+    k = max(1, a.steps)
     t = time.perf_counter()
     for _ in range(k):
-        step()
+        y = step()
     dt = time.perf_counter() - t
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, {"saliency_logits": y.numpy()})
     val = a.cpu_sample * k / dt
     sample = (f"{k} steps x {a.cpu_sample} images of the workload (the CPU path cannot finish {a.batch}-image steps "
               f"in minutes), all {cores} host threads")
@@ -195,7 +224,7 @@ def op_bytes(prog, op, n):
 
 
 def gpu_eager_baseline(a, dev, steps=5):
-    """BASELINE.md §4: eager PyTorch on the SAME B200 — the oracle's functional forward (exactly the reference module's
+    """BASELINE.md §4: eager PyTorch on the SAME GPU — the oracle's functional forward (exactly the reference module's
     ATen calls: F.conv2d / batch_norm / prelu / pooling / interpolate -> cuDNN / ATen kernels), fp32 and torch.autocast(fp16),
     NCHW as the reference runs.  A measured baseline, not the product: none of our kernels run here."""
     import torch
@@ -319,7 +348,7 @@ def train_record(a, world, rank, local, dev, steps=5, warmup=3):
     el = roofline.forward_elements(cfg, S, S)
     train_bytes = int(2.51 * el["module"]) * 4                  # 3*sum(I) + 2*sum(O) over modules (SURVEY 8d), fp32 storage
     peaks = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    peak = float(json.load(open(peaks))["hbm_gbs"]) if os.path.exists(peaks) else 6650.0
+    peak = float(json.load(open(peaks))["hbm_gbs"]) if os.path.exists(peaks) else H100_HBM_GBS
     ips, ips_e2e = B * world * steps / (ms * 1e-3), B * world * steps / (ms_e2e * 1e-3)
     bucket_bytes = int(tr.flat.bucket.numel() * 4)
     peak_gib = torch.cuda.max_memory_allocated(dev) / 2 ** 30
@@ -385,13 +414,20 @@ def run_ours(a):
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return float(ms.item())
 
+    last = [None]
+
+    def fwd():
+        last[0] = model(x_dev)
+
     with torch.no_grad():
-        fwd = lambda: model(x_dev)
         for _ in range(a.warmup):
             fwd()
         clocks = ClockSampler(local) if rank == 0 else None
         ms = timed(fwd, a.steps)
         clk = clocks.stop() if clocks else None
+        if a.dump_outputs and rank == 0:
+            dump_outputs(a.dump_outputs, {"saliency_logits": last[0].float().cpu().numpy()})
+        last[0] = None
         # end to end through host buffers (same call a user of the reference-facing API makes)
         e2e_fn = lambda: eng.forward_host(x_host, out=y_host, device=local)
         for _ in range(max(1, a.warmup // 2)):
@@ -400,7 +436,7 @@ def run_ours(a):
         # same, with the reference's pre / post-processing on the device (uint8 images in, uint8 maps out: test.py:68-98)
         ms_u8 = None
         if not a.no_extras:
-            xu8 = torch.randint(0, 256, (B, S, S, 3), dtype=torch.uint8).pin_memory()
+            xu8 = torch.randint(0, 256, (B, S, S, 3), dtype=torch.uint8, generator=torch.Generator().manual_seed(1235 + rank)).pin_memory()
             yu8 = torch.empty((B, S, S), dtype=torch.uint8).pin_memory()
             u8_fn = lambda: eng.forward_host_u8(xu8, out=yu8, device=local)
             for _ in range(max(1, a.warmup // 2)):
@@ -436,7 +472,7 @@ def run_ours(a):
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = H100_HBM_GBS, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
     prog = plan.prog
     # dominant KERNEL = the kernel (family) with the largest share of the step; its roofline is aggregated over its launches:
     # (sum of their algorithmic bytes) / (sum of their live CUDA-event durations) == mean bytes per launch / mean launch duration
@@ -462,14 +498,8 @@ def run_ours(a):
             print(f"{prog.ops[i].name:34s} {per_op[i]:8.3f} ms {100 * per_op[i] / tot:5.1f}%  {ob / per_op[i] / 1e6:8.1f} GB/s",
                   file=sys.stderr)
         print(f"sum of per-op times {tot:.3f} ms vs step {ms / a.steps:.3f} ms", file=sys.stderr)
-    # DRAM traffic of the dominant kernel: not measurable without a profiler, so it comes from the committed ncu capture of
-    # the same op / batch / size / dtype (profiles/traffic.json, written by scripts/ncu_traffic.sh), or stays null
+    # DRAM traffic of the dominant kernel is not measurable without a hardware profiler: not measured (null)
     traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        tj = json.load(open(tpath))
-        per = [tj.get(f"{a.model}:{prog.ops[i].name}:bs{B}:{S}x{S}:{a.dtype}") for i in dom_ops]
-        traffic = sum(per) if all(v is not None for v in per) else None
     out = {
         "metric": METRIC, "value": ips, "unit": UNIT, "n_gpus": world, "steps": a.steps, "warmup": a.warmup,
         "ms_per_step": ms / a.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -485,7 +515,7 @@ def run_ours(a):
                      "traffic": traffic, "kernel": dom, "kernel_share_of_step": dom_ms / sum(per_op), "kernel_launches_per_step": len(dom_ops),
                      "kernel_ms": dom_ms, "algorithmic_bytes": dom_bytes,
                      "note": "achieved = sum of the kernel's algorithmic bytes over its launches in one step / sum of their CUDA-event times; "
-                             "traffic = ncu dram bytes of the same launches (profiles/traffic.json)",
+                             "traffic = DRAM bytes of the same launches (needs a hardware profiler: not measured)",
                      "slowest_launch": {"op": prog.ops[top].name, "ms": per_op[top], "algorithmic_bytes": top_bytes,
                                         "achieved": top_bytes / (per_op[top] * 1e-3) / 1e9, "frac": top_bytes / (per_op[top] * 1e-3) / 1e9 / peak},
                      "by_kernel": {k_: {"ms": v_, "share": v_ / sum(per_op)} for k_, v_ in sorted(share.items(), key=lambda kv: -kv[1])},
@@ -564,7 +594,11 @@ def run_train(a):
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return float(ms.item())
 
-    step = lambda: tr.step(xd, td)
+    last = [None]
+
+    def step():
+        last[0] = tr.step(xd, td)
+
     e2e = lambda: tr.step(xh.to(dev, non_blocking=True), th.to(dev, non_blocking=True)).item()
     for _ in range(a.warmup):
         step()
@@ -573,12 +607,14 @@ def run_train(a):
     launches0 = train_ops.LAUNCHES
     ms = timed(step, a.steps)
     train_launches = train_ops.LAUNCHES - launches0          # csnet_train_* kernels of the timed steps (memsets not counted)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, {"loss": last[0].detach().float().reshape(1).cpu().numpy()})
     clk = clocks.stop() if clocks else None
     e2e()
     ms_e2e = timed(e2e, a.steps)
     if rank == 0:
         peaks = os.path.join(ROOT, "MEASURED_PEAKS.json")
-        peak = float(json.load(open(peaks))["hbm_gbs"]) if os.path.exists(peaks) else 6650.0
+        peak = float(json.load(open(peaks))["hbm_gbs"]) if os.path.exists(peaks) else H100_HBM_GBS
         el = roofline.forward_elements(cfg, S, S)
         ips, ips_e2e = B * world * a.steps / (ms * 1e-3), B * world * a.steps / (ms_e2e * 1e-3)
         train_bytes = int(2.51 * el["module"]) * 4          # 3*sum(I) + 2*sum(O) over modules (SURVEY 8d), fp32
@@ -629,13 +665,16 @@ def run_csf(a):
         for _ in range(a.warmup):
             m(x)
         clocks = ClockSampler(0)
-        ms = timed(lambda: m(x), a.steps)
+        last = [None]
+        ms = timed(lambda: last.__setitem__(0, m(x)), a.steps)
         clk = clocks.stop()
+        if a.dump_outputs:
+            dump_outputs(a.dump_outputs, {"saliency_logits": last[0].float().cpu().numpy()})
         ms_backbone = timed(lambda: m.backbone(x), a.steps)
     ips = B * a.steps / (ms * 1e-3)
     head_ms = (ms - ms_backbone) / a.steps
     peaks = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    tf = float(json.load(open(peaks))["bf16_tflops"]) if os.path.exists(peaks) else 1590.0
+    tf = float(json.load(open(peaks))["bf16_tflops"]) if os.path.exists(peaks) else H100_FP16_TFLOPS
     head_flops = 2 * 8.11e9 * (S / 352.0) ** 2 * B               # SURVEY: 8.11 GMAC per 352x352 image in the head
     print(json.dumps({
         "metric": "images/sec CSF+Res2Net50 fwd 352x352", "value": ips, "unit": UNIT, "n_gpus": 1, "steps": a.steps, "warmup": a.warmup,

@@ -1,5 +1,5 @@
 /*
- * csnet_b200.h — C ABI of libcsnet_b200.so, the B200 (sm_100a) CSNet forward/backward engine.
+ * csnet_b200.h — C ABI of libcsnet_b200.so, the H100 (sm_90a) CSNet forward/backward engine.
  *
  * The reference (ShangHua-Gao/SOD100K) has no FFI of its own: its hot path is Python calling
  * torch.nn.functional (ATen/cuDNN).  This header is the boundary a maintainer would bind instead of

@@ -1,6 +1,6 @@
 """GPU check of the streaming ILBlock kernel (csrc/il_stream.cuh): every qualifying block fused in isolation, the streaming
 kernel against the all-generic program (same inputs bit for bit), for several batch sizes / image sizes, then per-op times of the
-full fp16 program with the streaming kernel on and off.  Run on the B200 box:  python scripts/ils_check.py [--time]"""
+full fp16 program with the streaming kernel on and off.  Needs a GPU:  python scripts/ils_check.py [--time]"""
 import os
 import sys
 import json

@@ -12,7 +12,7 @@ for tag, dt, hw in (("csnet-L-x2", "fp32", (64, 96)), ("csnet-L-x1", "fp16", (64
         y = m(torch.from_numpy(synth.randn_images(2, hw[0], hw[1], 5)).cuda())
     torch.cuda.synchronize()
     print(tag, dt, hw, float(y.mean()))
-# 12 images at 224 x 224: enough row chunks for the streaming TMA / tcgen05 kernels (il_stream, mix_stream) to be selected
+# 12 images at 224 x 224: enough row chunks for the streaming TMA / wgmma kernels (il_stream, mix_stream) to be selected
 m, cfg, sd = checkpoints.build_from_npz("csnet-L-x2")
 m.cuda().eval().set_precision("fp16")
 with torch.no_grad():

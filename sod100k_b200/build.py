@@ -1,4 +1,4 @@
-"""Build libcsnet_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the repo)."""
+"""Build libcsnet_b200.so in-tree with nvcc for sm_90a (H100; no JIT cache: the library sits next to its sources)."""
 from __future__ import annotations
 
 import os
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libcsnet_b200.so")
 SOURCES = ["plan.cu", "train_ops.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-O3,-Wall", "-shared", "-cudart", "shared"]
 
 

@@ -86,10 +86,10 @@ template <> struct Pack<__half> {
     asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
                  : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(b));
   }
-  // acc += x * w with 16-bit x, w and fp32 accumulation in ONE instruction (sm_100 FHFMA): no operand conversions
+  // acc += x * w with 16-bit x, w and fp32 accumulation: the conversions are exact and the fp16 x fp16 product fits fp32
+  // exactly, so this is one rounding, as a fused mixed-precision FMA would give
   static __device__ __forceinline__ float fma16(uint16_t x, uint16_t w, float acc) {
-    asm("fma.rn.f32.f16 %0, %1, %2, %0;" : "+f"(acc) : "h"(x), "h"(w));
-    return acc;
+    return fmaf(__half2float(__ushort_as_half(x)), __half2float(__ushort_as_half(w)), acc);
   }
   static __device__ __forceinline__ uint16_t bits(float v) { return __half_as_ushort(__float2half_rn(v)); }
 };
@@ -109,8 +109,7 @@ template <> struct Pack<__nv_bfloat16> {
                  : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(b));
   }
   static __device__ __forceinline__ float fma16(uint16_t x, uint16_t w, float acc) {
-    asm("fma.rn.f32.bf16 %0, %1, %2, %0;" : "+f"(acc) : "h"(x), "h"(w));
-    return acc;
+    return fmaf(__bfloat162float(__ushort_as_bfloat16(x)), __bfloat162float(__ushort_as_bfloat16(w)), acc);
   }
   static __device__ __forceinline__ uint16_t bits(float v) { return __bfloat16_as_ushort(__float2bfloat16_rn(v)); }
 };
@@ -224,8 +223,8 @@ __device__ __forceinline__ void dw_task(int task, const uint16_t* in, uint16_t* 
   const int gi = task % G, rest = task / G;
   const int run = rest % NR, c = rest / NR;
   const int x = 4 * (GEO::G0 + gi), ra = GEO::R0 + run * RUN;
-  // fp16 planes: the 9 taps run as the mixed-precision FMA (Pack<T>::fma16: 16-bit x 16-bit + fp32 in one instruction), so
-  // no operand is converted; the weights are rounded to fp16 for it (measured: no change of the fp16 error figures).
+  // fp16 planes: the 9 taps run as Pack<T>::fma16 (16-bit x 16-bit + fp32, one rounding) with the weights packed as
+  // fp16 pairs, which halves their registers (measured: no change of the fp16 error figures).
   // bf16 planes keep fp32 weights and converted operands — 8-bit-mantissa weights cost accuracy there.
   constexpr bool kMixed = std::is_same<T, __half>::value;
   float wf[9];
@@ -305,7 +304,7 @@ inline size_t il_smem_bytes(const IlArgs& A, int NPH, int NPL) {
   return halves * 2 + 128 /*base alignment*/ + 128 /*mbarrier + front guard*/ + 128 /*bufAh size round-up*/ + 128 /*tail guard*/;
 }
 
-// NT threads per CTA (512, one CTA per SM; 256 x 2 CTAs, 768 and 1024 were measured and are no faster, profiles/r01_f).
+// NT threads per CTA (512, one CTA per SM).
 template <typename T, int TH, int TW, int NT = kIlThreads>
 __global__ void __launch_bounds__(NT, NT <= 256 ? 2 : 1)
 il_block_kernel(const __grid_constant__ IlArgs A, const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmL) {

@@ -1,4 +1,4 @@
-// il_stream.cuh — the 1x1-kind ILBlock as ONE persistent, streaming kernel on the Blackwell data path
+// il_stream.cuh — the 1x1-kind ILBlock as ONE persistent, streaming kernel on the Hopper data path (TMA + wgmma)
 // (reference: ILBlock.forward, CSNet/model/csnet.py:72-76 = gOctaveCBR :778-792 over gOctaveConv.forward :664-726,
 // then two SimplifiedGOctConvBR.forward :838-851).
 //
@@ -11,9 +11,9 @@
 //   resample   bilinear x2 of x_l -> slots [Chi, Chi+Cli) of the hi chunk (lo -> hi path, csnet.py:702-707; the
 //              up-sample commutes with the 1x1 conv), max-pool 2x2 of x_h -> slots [Cli, Cli+Chi) of the lo chunk
 //              (hi -> lo path, :709-712).
-//   GEMM       one elected thread issues tcgen05.mma (kind::f16, M = 128 pixels, N = ru16(Cout), K = 16 per
-//              instruction) per 16 pixel groups; fp32 accumulators of the whole chunk live in TMEM.
-//   epilogue   tcgen05.ld (a thread = a pixel), + bias, PReLU, 16-bit, written IN PLACE over the chunk (T1).
+//   GEMM       a warpgroup issues wgmma.mma_async (f16 x f16 -> f32, M = 64 pixels, N = ru16(Cout), K = 16 per
+//              instruction) per 8 pixel groups straight from the shared-memory tiles; fp32 accumulators in registers.
+//   epilogue   from the accumulator fragment: + bias, PReLU, 16-bit, written IN PLACE over the chunk (T1).
 //   dw tail    a thread owns (channel, 8-pixel column) for the whole walk and keeps the 3-row windows of T1 and T2
 //              in registers: dw3x3+BN+PReLU twice with no halo recomputation in y, no shared-memory round trip for
 //              T2, 16-byte coalesced stores of the block output.  (mixed-precision FMA: fp16 x fp16 + fp32.)
@@ -25,8 +25,7 @@
 //
 // An image is cut into `ns` column strips of gsn 8-pixel groups (gsn even); a CTA's tile of a strip carries one halo
 // group on each side when ns > 1 (hl = 1: the TMA box starts one group early, out-of-image groups arrive as zeros).
-// Narrow strips let two CTAs share an SM (<= 113 KB shared memory, <= 256 TMEM columns each), so one CTA's waits
-// (TMA, MMA, barriers) are filled by the other's depthwise phase.  No row halo is ever re-read from HBM (except one
+// Narrow strips shrink a CTA's shared memory and threads.  No row halo is ever re-read from HBM (except one
 // warm-up chunk where a CTA's range starts inside an image); the work split is a flat division of the
 // N * ns * H/4 chunks over the CTAs.  Needs W % 16 == 0, H % 4 == 0, K = Chi + Cli <= 64.  Other shapes: il_block.cuh.
 #pragma once
@@ -52,7 +51,6 @@ struct IlsArgs {
   int32_t GH, GL;                     // pixel groups per image row: W/8, W/16
   int32_t ns, gsn, hl;                // column strips per image, hi groups per strip (even), halo groups per side (0 / 1)
   int32_t GR, GLR;                    // groups per row of a CTA's tile: gsn + 2 hl, gsn/2 + 2 hl
-  int32_t tmem_cols;                  // TMEM columns to allocate (power of two >= the chunk's accumulators)
   int32_t Ci, BW;                     // stem form: image channels; width in floats of an image block in shared memory (8 GR + 8)
   int32_t off_xlo;                    // stem form: the lo chunk's GEMM operand buffer
   int32_t cpi, total_chunks;          // chunks per image strip (H/4), N * ns * cpi
@@ -84,22 +82,69 @@ __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
     if (clock64() - t0 > 4000000000LL) __trap();
   }
 }
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  // shared-memory matrix descriptor, no swizzle, version 1 (sm_100): start / LBO / SBO in 16-byte units
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  // wgmma shared-memory matrix descriptor, no swizzle: start / LBO / SBO in 16-byte units.  LBO = the stride between
+  // core matrices along K, SBO = along M / N (for the MN-major A operand as for the K-major B operand).
   return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46);
+         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32);
 }
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-               ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
+// wgmma.m64nNk16, fp32 += f16 x f16: A (64 pixels x 16 channels) MN-major from shared memory (transposed: pixels are the
+// contiguous dimension of a core matrix), B (N output channels x 16) K-major; d: the warpgroup's accumulator fragment.
+template <int N> struct Wgmma;
+template <> struct Wgmma<16> {
+  static __device__ __forceinline__ void mma(float (&d)[8], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 1, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                 : "l"(da), "l"(db), "r"(acc));
+  }
+};
+template <> struct Wgmma<32> {
+  static __device__ __forceinline__ void mma(float (&d)[16], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 1, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "l"(da), "l"(db), "r"(acc));
+  }
+};
+template <> struct Wgmma<48> {
+  static __device__ __forceinline__ void mma(float (&d)[24], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %26, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, 1, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+                 : "l"(da), "l"(db), "r"(acc));
+  }
+};
+template <> struct Wgmma<64> {
+  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 1, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(da), "l"(db), "r"(acc));
+  }
+};
+template <> struct Wgmma<80> {
+  static __device__ __forceinline__ void mma(float (&d)[40], uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %42, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 1, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+                 : "l"(da), "l"(db), "r"(acc));
+  }
+};
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit_wait() {
+  asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory");
+  asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory");
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
+__device__ __forceinline__ void warpgroup_bar(int wg) { asm volatile("bar.sync %0, 128;\n" ::"r"(1 + wg) : "memory"); }
+// One 64-pixel block of the warpgroup: d = A[64][K16] . B[N][K16]^T over K16 / 16 instructions.
+template <int N>
+__device__ __forceinline__ void wgmma_block(float (&d)[N / 2], uint64_t da, uint64_t db, int K16) {
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+  wgmma_fence();
+  for (int ks = 0; ks < (K16 >> 4); ++ks) Wgmma<N>::mma(d, da + (uint64_t)(16 * ks), db + (uint64_t)(16 * ks), ks > 0);
+  wgmma_commit_wait();
 }
 __device__ __forceinline__ uint32_t lds32(uint32_t a) { uint32_t v; asm volatile("ld.shared.b32 %0, [%1];\n" : "=r"(v) : "r"(a)); return v; }
 __device__ __forceinline__ uint2 lds64(uint32_t a) { uint2 v; asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];\n" : "=r"(v.x), "=r"(v.y) : "r"(a)); return v; }
@@ -173,46 +218,50 @@ __device__ __forceinline__ void ils_dw_push(uint32_t (&t1)[2][6], uint32_t (&t2)
   for (int i = 0; i < 5; ++i) { t2[0][i] = t2[1][i]; t2[1][i] = q[i]; }
 }
 
-__device__ __forceinline__ void tmem_ld_16x256b_x2(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.16x256b.x2.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
 __device__ __forceinline__ void stsm_x4_trans(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};\n" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
 
-// Epilogue of one warp's 32 accumulator rows (= 32 pixels = 4 pixel groups, TMEM lanes [32 q, 32 q + 32)) of a 128-pixel
-// block: tcgen05.ld in the 16x256b shape hands a thread the mma-style fragment (row lane/4 and lane/4 + 8, columns
-// 2 (lane % 4) + {0, 1} of every 8-column slab) = pixel rows x channel pairs; + bias, PReLU, pack to 16 bits, then
-// stmatrix.trans writes each 8 px x 8 channel fragment as 8 channel rows of 8 contiguous pixels — exactly the
-// [group][slot][8 px] tile.  16 channels x 16 pixels per round trip.  g0: first pixel group of the warp's 4,
-// ngroups: groups of the chunk (later ones are MMA padding: stored to `dummy`), gstride = slots * 16 bytes.
-// eb / es: shared-memory tables of bias and (slope - 1) per channel.
-template <typename T>
-__device__ __forceinline__ void ils_epilogue_warp(uint32_t taddr, uint32_t tile, uint32_t gstride, int g0, int ngroups, int C,
-                                                  uint32_t eb, uint32_t es, uint32_t dummy, int lane) {
+// GEMM and epilogue of one 64-pixel block (8 pixel groups) by a warpgroup.  Warp qd of the group holds accumulator rows
+// [16 qd, 16 qd + 16) = pixel groups g0, g0 + 1 (g0 = 8 b + 2 qd); the m64nNk16 fragment gives a thread rows lane/4 and
+// lane/4 + 8, columns 2 (lane % 4) + {0, 1} of every 8-column slab = pixel rows x channel pairs.  + bias, PReLU, pack to 16
+// bits, then stmatrix.trans writes each 8 px x 8 channel fragment as 8 channel rows of 8 contiguous pixels — exactly the
+// [group][slot][8 px] tile.  ngroups: groups of the chunk (later ones are MMA padding: stored to `dummy`), gstride = slots *
+// 16 bytes.  eb / es: shared-memory tables of bias and (slope - 1) per channel.  The tile may be the A operand itself (T1
+// written in place): the warpgroup barrier keeps every warp's stores behind the whole group's MMAs.
+template <typename T, int N>
+__device__ __forceinline__ void ils_block(uint64_t da, uint64_t db, int K16, int wg, uint32_t tile, uint32_t gstride, int g0, int ngroups,
+                                          uint32_t eb, uint32_t es, uint32_t dummy, int lane) {
+  float d[N / 2];
+  wgmma_block<N>(d, da, db, K16);
+  warpgroup_bar(wg);
   const int q = lane & 3, mrow = lane & 7, mat = lane >> 3;
-#pragma unroll 1
-  for (int cc = 0; cc * 16 < C; ++cc) {
+#pragma unroll
+  for (int cc = 0; cc < N / 16; ++cc) {
     const uint32_t co = (uint32_t)(cc * 16 + 2 * q) * 4u;
     const uint2 bA = lds64(eb + co), bB = lds64(eb + co + 32u), sA = lds64(es + co), sB = lds64(es + co + 32u);
     const float b0 = __uint_as_float(bA.x), b1 = __uint_as_float(bA.y), b2 = __uint_as_float(bB.x), b3 = __uint_as_float(bB.y);
     const float s0 = __uint_as_float(sA.x), s1 = __uint_as_float(sA.y), s2 = __uint_as_float(sB.x), s3 = __uint_as_float(sB.y);
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      uint32_t r[8];
-      tmem_ld_16x256b_x2(taddr + ((uint32_t)(16 * h) << 16) + (uint32_t)(cc * 16), r);
-      const uint32_t m0 = Pack<T>::from_f2(prelu_m1(__uint_as_float(r[0]) + b0, s0), prelu_m1(__uint_as_float(r[1]) + b1, s1));
-      const uint32_t m1 = Pack<T>::from_f2(prelu_m1(__uint_as_float(r[2]) + b0, s0), prelu_m1(__uint_as_float(r[3]) + b1, s1));
-      const uint32_t m2 = Pack<T>::from_f2(prelu_m1(__uint_as_float(r[4]) + b2, s2), prelu_m1(__uint_as_float(r[5]) + b3, s3));
-      const uint32_t m3 = Pack<T>::from_f2(prelu_m1(__uint_as_float(r[6]) + b2, s2), prelu_m1(__uint_as_float(r[7]) + b3, s3));
-      // matrix `mat` of the x4 store: pixel group g0 + 2h + (mat & 1), channels 16 cc + 8 (mat >> 1) ..; this lane addresses row mrow
-      const int pg = g0 + 2 * h + (mat & 1);
-      const uint32_t addr = pg < ngroups ? tile + (uint32_t)pg * gstride + (uint32_t)(cc * 16 + 8 * (mat >> 1) + mrow) * 16u
-                                         : dummy + (uint32_t)(mat * 8 + mrow) * 16u;
-      stsm_x4_trans(addr, m0, m1, m2, m3);
-    }
+    const float* r = d + 8 * cc;
+    const uint32_t m0 = Pack<T>::from_f2(prelu_m1(r[0] + b0, s0), prelu_m1(r[1] + b1, s1));
+    const uint32_t m1 = Pack<T>::from_f2(prelu_m1(r[2] + b0, s0), prelu_m1(r[3] + b1, s1));
+    const uint32_t m2 = Pack<T>::from_f2(prelu_m1(r[4] + b2, s2), prelu_m1(r[5] + b3, s3));
+    const uint32_t m3 = Pack<T>::from_f2(prelu_m1(r[6] + b2, s2), prelu_m1(r[7] + b3, s3));
+    // matrix `mat` of the x4 store: pixel group g0 + (mat & 1), channels 16 cc + 8 (mat >> 1) ..; this lane addresses row mrow
+    const int pg = g0 + (mat & 1);
+    const uint32_t addr = pg < ngroups ? tile + (uint32_t)pg * gstride + (uint32_t)(cc * 16 + 8 * (mat >> 1) + mrow) * 16u
+                                       : dummy + (uint32_t)(mat * 8 + mrow) * 16u;
+    stsm_x4_trans(addr, m0, m1, m2, m3);
+  }
+}
+template <typename T>
+__device__ __forceinline__ void ils_block_n(int N, uint64_t da, uint64_t db, int K16, int wg, uint32_t tile, uint32_t gstride, int g0,
+                                            int ngroups, uint32_t eb, uint32_t es, uint32_t dummy, int lane) {
+  switch (N) {
+    case 16: ils_block<T, 16>(da, db, K16, wg, tile, gstride, g0, ngroups, eb, es, dummy, lane); break;
+    case 32: ils_block<T, 32>(da, db, K16, wg, tile, gstride, g0, ngroups, eb, es, dummy, lane); break;
+    case 48: ils_block<T, 48>(da, db, K16, wg, tile, gstride, g0, ngroups, eb, es, dummy, lane); break;
+    default: ils_block<T, 64>(da, db, K16, wg, tile, gstride, g0, ngroups, eb, es, dummy, lane); break;
   }
 }
 
@@ -225,9 +274,8 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
   const uint32_t XL = sbase + A.off_xl, XH = sbase + A.off_xh, T1L = sbase + A.off_t1l, WBH = sbase + A.off_wbh,
                  WBL = sbase + A.off_wbl, BAR = sbase + A.off_bar, ZERO = sbase + A.off_zero;
   uint8_t* gbase = smem_raw + (sbase - smem_u32(smem_raw));      // generic pointer to the same place
-  // barriers: [0,2) hi stage full, [2,5) lo stage full; +64 the TMEM base slot; +128: one per accumulator block (16)
-  const uint32_t bar_h = BAR, bar_l = BAR + 16, bar_m = BAR + 128;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(gbase + A.off_bar + 64);
+  // barriers: [0,2) hi stage full, [2,5) lo stage full
+  const uint32_t bar_h = BAR, bar_l = BAR + 16;
   const uint32_t EPI = sbase + A.off_epi, DUMMY = EPI + 1024;     // bias_h, sm1_h, bias_l, sm1_l (64 floats each); scratch rows
 
   const int H = A.H, W = A.W, Hl = H >> 1, Wl = W >> 1;
@@ -239,12 +287,7 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
   // ---- one-time setup -----------------------------------------------------------------------------------
   if (tid == 0) {
     for (int i = 0; i < 6; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;\n" ::"r"(BAR + 8 * i) : "memory");
-    for (int i = 0; i < 16; ++i) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;\n" ::"r"(bar_m + 8 * i) : "memory");
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(BAR + 64), "r"(A.tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
   }
   // weights -> K-major B operand: core matrices [n group][k group][8 n][8 k]
   {
@@ -281,10 +324,7 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
     }
   }
   asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  const uint32_t tmem = *tmem_slot;
 
   // depthwise-tail role of this thread (fixed for the whole kernel): a channel and an 8-pixel column
   // tail tasks are packed: threads [0, Cho * gsn) own a hi (channel, column), the next Clo * gsn / 2 a lo one
@@ -317,16 +357,15 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
   const uint32_t dw_off = (uint32_t)((dg + hl) * Sd + dc) * 16u, dw_rowstep = (uint32_t)((dw_hi ? GR : GLR) * Sd) * 16u;
   const int Gimg = dw_hi ? GH : GL;                       // groups per image row of this role
 
-  const uint32_t idesc_h = (1u << 4) | (1u << 15) | ((uint32_t)(NH >> 3) << 17) | (8u << 24);   // f16 x f16 -> f32, A MN-major, M = 128
-  const uint32_t idesc_l = (1u << 4) | (1u << 15) | ((uint32_t)(NL >> 3) << 17) | (8u << 24);
-  const int nbh = (4 * GR + 15) >> 4, nbl = NL > 0 ? (2 * GLR + 15) >> 4 : 0;
+  const int nbh = (4 * GR + 7) >> 3, nbl = NL > 0 ? (2 * GLR + 7) >> 3 : 0;     // 64-pixel GEMM blocks of a chunk
+  const uint64_t db_h = gmma_desc(WBH, 128u, (uint32_t)(K16 >> 3) * 128u), db_l = gmma_desc(WBL, 128u, (uint32_t)(K16 >> 3) * 128u);
   const uint32_t hi_tx = (uint32_t)(64 * SH * GR), lo_tx = kStem ? (uint32_t)(A.BW * 4 * A.Ci * 4) : (uint32_t)(32 * SL * GLR);
   const uint32_t XLO = sbase + A.off_xlo;
 
   // ---- the CTA's range of the (image, chunk) sequence ------------------------------------------------
   int ra = (int)((long long)blockIdx.x * A.total_chunks / gridDim.x);
   const int rb = (int)((long long)(blockIdx.x + 1) * A.total_chunks / gridDim.x);
-  uint32_t hq = 0, lq = 0, mq = 0;                       // running counts: hi loads, lo loads, MMA commits
+  uint32_t hq = 0, lq = 0;                               // running counts: hi loads, lo loads
   long long tph[8] = {0, 0, 0, 0, 0, 0, 0, 0}, tlast = clock64();
   const bool timing = kTiming && A.dbg != nullptr && tid == 0;
 #define ILS_MARK(i) do { if (kTiming && timing) { const long long t_ = clock64(); tph[i] += t_ - tlast; tlast = t_; } } while (0)
@@ -514,43 +553,27 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
       asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");    // generic writes -> visible to the tensor core / TMA
       __syncthreads();                                                    // (A)
       ILS_MARK(2);
-      // ---- 3. next loads (one thread of the last warp); the chunk's MMAs: warp b's elected lane issues block b ----
+      // ---- 3. next loads (one thread of the last warp) ------------------------------------------------------
       if (warp == nwarps - 1 && lane == 0) {
         asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
         if (!kStem && c >= c0 + 1 && c + 1 <= c1) issue_hi(c + 1);       // stage of chunk c-1: its T1 was consumed
         if (c + 2 <= cl1) issue_lo(c + 2);                               // stage of lo chunk c-1: last read by this chunk's up-sample
       }
-      if (lane == 0) {
-        for (int b = warp; b < nbh + nbl; b += nwarps) {
-          asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-          const bool hb = b < nbh;
-          const int lb = hb ? b : b - nbh, S_ = hb ? SH : SL;
-          const uint64_t da = umma_desc((hb ? xh : xl) + (uint32_t)(lb * 16 * S_) * 16u, 128u, (uint32_t)S_ * 16u);
-          const uint64_t db = umma_desc(hb ? WBH : WBL, 128u, (uint32_t)(K16 >> 3) * 128u);
-          const uint32_t tm = tmem + (uint32_t)(hb ? lb * NH : nbh * NH + lb * NL), idesc = hb ? idesc_h : idesc_l;
-          for (int ks = 0; ks < (K16 >> 4); ++ks) umma_f16(tm, da + (uint64_t)(16 * ks), db + (uint64_t)(16 * ks), idesc, ks > 0);
-          asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar_m + 8u * b) : "memory");
-        }
-      }
-      __syncwarp();
       ILS_MARK(3);
-      // ---- 4. epilogue: TMEM -> bias, PReLU, 16-bit -> T1 (hi: in place over the chunk; lo: its own buffer) ----
+      // ---- 4. GEMM + epilogue: warpgroup w takes the 64-pixel blocks w, w + wgs, ..; fp32 accumulators in registers ->
+      //         bias, PReLU, 16-bit -> T1 (hi: in place over the block's own pixel groups; lo: its own buffer) ----------------
       if (warp < (nwarps & ~3)) {
-        const int qd = warp & 3, wstep = nwarps >> 2;
-        for (int b = warp >> 2; b < nbh + nbl; b += wstep) {
-          mbar_wait_a(bar_m + 8u * b, mq & 1u);                      // the block's MMAs (and all earlier ones) have completed
-          asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
+        const int wg = warp >> 2, qd = warp & 3, wgs = nwarps >> 2;
+        for (int b = wg; b < nbh + nbl; b += wgs) {
           if (b < nbh)
-            ils_epilogue_warp<T>(tmem + ((uint32_t)(qd * 32) << 16) + (uint32_t)(b * NH), xh, (uint32_t)SH * 16u, b * 16 + qd * 4, 4 * GR, Cho,
-                                 EPI, EPI + 256u, DUMMY, lane);
+            ils_block_n<T>(NH, gmma_desc(xh + (uint32_t)(b * 8 * SH) * 16u, 128u, (uint32_t)SH * 16u), db_h, K16, wg, xh, (uint32_t)SH * 16u,
+                           b * 8 + qd * 2, 4 * GR, EPI, EPI + 256u, DUMMY, lane);
           else
-            ils_epilogue_warp<T>(tmem + ((uint32_t)(qd * 32) << 16) + (uint32_t)(nbh * NH + (b - nbh) * NL), T1L, (uint32_t)ST * 16u,
-                                 (b - nbh) * 16 + qd * 4, 2 * GLR, Clo, EPI + 512u, EPI + 768u, DUMMY, lane);
+            ils_block_n<T>(NL, gmma_desc(xl + (uint32_t)((b - nbh) * 8 * SL) * 16u, 128u, (uint32_t)SL * 16u), db_l, K16, wg, T1L,
+                           (uint32_t)ST * 16u, (b - nbh) * 8 + qd * 2, 2 * GLR, EPI + 512u, EPI + 768u, DUMMY, lane);
         }
       }
-      ++mq;
       ILS_MARK(4);
-      asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
       __syncthreads();                                                    // (B)
       ILS_MARK(5);
       // ---- 5. depthwise tail over the chunk's rows --------------------------------------------------------
@@ -588,9 +611,6 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
     for (int i = 0; i < 8; ++i) A.dbg[(size_t)blockIdx.x * 8 + i] = (unsigned long long)tph[i];
   }
 #undef ILS_MARK
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem), "r"(A.tmem_cols) : "memory");
 }
 
 }  // namespace csnet

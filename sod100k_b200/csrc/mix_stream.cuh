@@ -1,4 +1,4 @@
-// mix_stream.cuh — a 1x1 CSNET_OP_MIX / CSNET_OP_MIXPROJ op as a persistent, warp-specialised TMA -> tcgen05 -> epilogue
+// mix_stream.cuh — a 1x1 CSNET_OP_MIX / CSNET_OP_MIXPROJ op as a persistent, warp-specialised TMA -> wgmma -> epilogue
 // pipeline (reference: the 1x1 gOctaveCBR calls of CSFHead.forward, CSNet/model/csnet.py:202-206 over gOctaveConv.forward
 // :664-726, and cls_layer :383 folded into the epilogue).
 //
@@ -7,12 +7,12 @@
 //   * every conv path is a plain 1x1 over a 16-bit tensor at the destination's resolution (W % 8 == 0).  A 2-row chunk of
 //     each input arrives by cp.async.bulk.tensor.5d in the tensor-core operand layout [row][8-px group][slot][8 px]
 //     (channel slots past C zero-filled = the K padding): the threads never touch the operands.
-//   * warp 0 (one lane) is the TMA producer over a ring of stages; warp 1 (one lane) issues tcgen05.mma: M = 128 pixels,
-//     N = ru16(Cout), K = 16 per instruction, the paths of the op accumulate into the same TMEM columns (K-concatenation);
-//     accumulators are double-buffered in TMEM (tcgen05.commit -> mbarrier hands a chunk to the epilogue and frees its stage).
-//   * epilogue warps (a thread = a pixel, tcgen05.ld 32x32b): bias, the op's resample-add paths (fp32 low-resolution conv
-//     results of the up-paths, gathered bilinearly from L2), PReLU, then either 16-bit stores of the Cout planes or the
-//     projection onto one fp32 channel (cls_layer) — the Cout-channel tensor is never written.
+//   * warp 0 (one lane) is the TMA producer over a ring of stages; kMsGroups consumer warpgroups share the 64-pixel blocks
+//     of each chunk: wgmma.mma_async (M = 64 pixels, N = ru16(Cout), K = 16 per instruction, the paths of the op accumulate
+//     into the same registers = K-concatenation), then the epilogue from the accumulator fragment: bias, the op's
+//     resample-add paths (fp32 low-resolution conv results of the up-paths, gathered bilinearly from L2), PReLU, then
+//     either stores of the Cout planes or the projection onto one fp32 channel (cls_layer) — the Cout-channel tensor is
+//     never written.  While one warpgroup runs its epilogue, the others' MMAs and the producer's loads are in flight.
 // 3x3 form (k3: every conv path a 3x3, pad 1 — the stage-entry gOctaveCBR of stride-2 ILBlocks, csnet.py:60-71 with the
 // avg-pooled inputs): the TMA box carries one halo row above and below (zero fill = the conv padding), two builder warps
 // derive the x-1 / x+1 shifted copies of the tile in shared memory (one 16-byte funnel shift per group), and the nine taps are
@@ -24,7 +24,7 @@
 namespace csnet {
 
 constexpr int kMsMaxIn = 3, kMsMaxRs = 2, kMsMaxC = 80, kMsRows = 2;
-constexpr int kMsEpiGroups = 5, kMsEpiWarps = 4 * kMsEpiGroups, kMsThreads = (4 + kMsEpiWarps) * 32;   // warps 0 / 1: TMA / MMA; 2, 3 idle; 4..: epilogue
+constexpr int kMsGroups = 3, kMsThreads = (4 + 4 * kMsGroups) * 32;   // warp 0: TMA; 2, 3: 3x3 builders; 4..: consumer warpgroups
 
 struct MsArgs {
   void* dst;
@@ -35,8 +35,7 @@ struct MsArgs {
   int32_t has_proj, has_slope, dst_f32;
   int32_t n_in, cin[kMsMaxIn], cout0[kMsMaxIn], cout[kMsMaxIn], S[kMsMaxIn], K16[kMsMaxIn], in_off[kMsMaxIn];
   int32_t n_rs, r_dtype[kMsMaxRs], r_up[kMsMaxRs], r_H[kMsMaxRs], r_W[kMsMaxRs], r_C[kMsMaxRs], r_c0[kMsMaxRs], r_cout0[kMsMaxRs], r_n[kMsMaxRs];
-  int32_t N, H, W, C, NN, G, nb;        // destination dims; NN = ru16(C); G = W / 8; nb = accumulator blocks per chunk
-  int32_t n_acc;                        // accumulator buffers in TMEM (chunks between the MMA issuer and the epilogue)
+  int32_t N, H, W, C, NN, G, nb;        // destination dims; NN = ru16(C); G = W / 8; nb = 64-pixel GEMM blocks per chunk
   int32_t k3, copy_bytes[kMsMaxIn];     // 3x3 form; bytes of one of the three copies (centre, x-1, x+1) of input i's tile
   int32_t cpi, total_chunks, n_stages, stage_bytes, tx_bytes;
   int32_t off_stage, off_wb[kMsMaxIn], off_bar, off_tab, smem_bytes;
@@ -61,68 +60,106 @@ __device__ __forceinline__ MsTap ms_tap(int Hs, int Ws, int up, int oy, int ox) 
   return t;
 }
 
-// Epilogue of the (chunk, block) tasks of one warp: a thread = a pixel (TMEM lane).  NRS resample-add paths (fp32 sources),
-// PROJ: project the C channels onto one fp32 value instead of storing them.  tab: shared-memory float4 {bias, slope-1, proj, 0}.
-template <typename T, int NRS, bool PROJ>
-__device__ __forceinline__ void ms_epilogue(const MsArgs& A, uint32_t tmem, uint32_t tab, uint32_t bar_tfull, uint32_t bar_tempty, int ra, int rb,
-                                            int q, int grp, int lane) {
-  const int H = A.H, W = A.W, C = A.C, G = A.G, nb = A.nb, NN = A.NN, NA = A.n_acc;
+// Consumer warpgroup `wg`: the (chunk, block) tasks t = k * nb + blk with t % kMsGroups == wg.  A task = one 64-pixel
+// block: wgmma over every conv path (and tap) of the op into one fp32 accumulator fragment, then the epilogue from the
+// fragment (rows lane/4 and lane/4 + 8 of the warp's 16 pixels, channel pairs 2 (lane % 4) + {0, 1} of every 8-channel slab):
+// bias, NRS resample-add paths (fp32 sources), PReLU, then 16-bit (or fp32) stores of the C planes, or (PROJ) the projection
+// onto one fp32 channel, summed over the four lanes that share a pixel.  tab: shared-memory float4 {bias, slope-1, proj, 0}.
+// Every warpgroup waits for every chunk and releases its stage once (bar_empty counts kMsGroups arrivals), so the
+// barriers' phases never run ahead of a warpgroup that has no task in a chunk.
+template <typename T, int NRS, bool PROJ, int NN>
+__device__ __forceinline__ void ms_consume(const MsArgs& A, uint32_t sbase, uint32_t STG, uint32_t tab, uint32_t bar_ready, uint32_t bar_empty,
+                                           int ra, int rb, int wg, int qd, int lane) {
+  const int H = A.H, W = A.W, C = A.C, G = A.G, nb = A.nb, NS = A.n_stages, taps = A.k3 ? 9 : 1;
   const size_t plane = (size_t)H * W;
+  const int q = lane & 3;
   for (int idx = ra, k = 0; idx < rb; ++idx, ++k) {
-    const int a = k % NA, n = idx / A.cpi, c = idx - n * A.cpi;
-    bool waited = false;
+    const int s = k % NS, n = idx / A.cpi, c = idx - n * A.cpi;
+    const uint32_t st = STG + (uint32_t)s * (uint32_t)A.stage_bytes;
+    mbar_wait_a(bar_ready + 8 * s, (uint32_t)(k / NS) & 1u);
     for (int blk = 0; blk < nb; ++blk) {
-      if ((k * nb + blk) % kMsEpiGroups != grp) continue;                  // warp-uniform
-      if (!waited) {
-        mbar_wait_a(bar_tfull + 8 * a, (uint32_t)(k / NA) & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-        waited = true;
-      }
-      const int p = blk * 128 + q * 32 + lane, pg = p >> 3;
-      const bool valid = pg < kMsRows * G;
-      const int r = pg / G, g = pg - r * G;
-      const int y = valid ? c * kMsRows + r : 0, x = valid ? 8 * g + (p & 7) : 0;
-      MsTap tp[NRS > 0 ? NRS : 1];
-      const float* rs[NRS > 0 ? NRS : 1];
-      size_t rplane[NRS > 0 ? NRS : 1];
+      if ((k * nb + blk) % kMsGroups != wg) continue;                      // warpgroup-uniform
+      float d[NN / 2];
 #pragma unroll
-      for (int j = 0; j < NRS; ++j) {
-        tp[j] = ms_tap(A.r_H[j], A.r_W[j], A.r_up[j], y, x);
-        rplane[j] = (size_t)(A.r_H[j] * A.r_W[j]);
-        rs[j] = reinterpret_cast<const float*>(A.rsrc[j]) + ((size_t)n * A.r_C[j] + (size_t)A.r_c0[j]) * rplane[j];
-      }
-      float proj_acc = 0.f;
-      uint16_t* d16 = reinterpret_cast<uint16_t*>(A.dst) + (size_t)n * C * plane + (size_t)y * W + x;
-      float* d32 = reinterpret_cast<float*>(A.dst) + (size_t)n * C * plane + (size_t)y * W + x;
-      const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * nb * NN + blk * NN);
-      for (int cc = 0; cc * 16 < C; ++cc) {
-        uint32_t rg[16];
-        tmem_ld16(taddr + (uint32_t)(cc * 16), rg);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int ch = cc * 16 + j;                                     // channels >= C: zero weights, zero tables -> harmless work
-          const uint4 t4 = lds128(tab + (uint32_t)ch * 16u);
-          float v = __uint_as_float(rg[j]) + __uint_as_float(t4.x);
-#pragma unroll
-          for (int t = 0; t < NRS; ++t) {
-            if (ch < A.r_n[t]) {                                          // (resample-add paths cover channels [0, r_n): checked by the host)
-              const float* s_ = rs[t] + (size_t)ch * rplane[t];
-              v += tp[t].w00 * __ldg(s_ + tp[t].o00) + tp[t].w01 * __ldg(s_ + tp[t].o01) + tp[t].w10 * __ldg(s_ + tp[t].o10) + tp[t].w11 * __ldg(s_ + tp[t].o11);
-            }
-          }
-          v = prelu_m1(v, __uint_as_float(t4.y));
-          if (PROJ) proj_acc = fmaf(__uint_as_float(t4.z), v, proj_acc);
-          else if (valid && ch < C) {
-            if (A.dst_f32) d32[(size_t)ch * plane] = v;
-            else d16[(size_t)ch * plane] = Pack<T>::bits(v);
+      for (int i = 0; i < NN / 2; ++i) d[i] = 0.f;
+      wgmma_fence();
+      uint32_t acc = 0;
+      for (int i = 0; i < A.n_in; ++i) {
+        for (int tap = 0; tap < taps; ++tap) {
+          // 3x3: tap (ky, kx) reads copy kx (x-1 / centre / x+1 = copies 1 / 0 / 2) ky tile rows down
+          const int ky = tap / 3, kx = tap - 3 * ky, cp = kx == 1 ? 0 : (kx == 0 ? 1 : 2);
+          const uint32_t abase = st + (uint32_t)A.in_off[i] + (A.k3 ? (uint32_t)cp * (uint32_t)A.copy_bytes[i] + (uint32_t)(ky * G * A.S[i]) * 16u : 0u);
+          const uint64_t da = gmma_desc(abase + (uint32_t)(blk * 8 * A.S[i]) * 16u, 128u, (uint32_t)A.S[i] * 16u);
+          const uint64_t db = gmma_desc(sbase + (uint32_t)A.off_wb[i] + (uint32_t)(tap * NN * A.K16[i] * 2), 128u, (uint32_t)(A.K16[i] >> 3) * 128u);
+          for (int ks = 0; ks < (A.K16[i] >> 4); ++ks) {
+            Wgmma<NN>::mma(d, da + (uint64_t)(16 * ks), db + (uint64_t)(16 * ks), acc);
+            acc = 1;
           }
         }
       }
-      if (PROJ && valid) reinterpret_cast<float*>(A.dst)[((size_t)n * H + y) * W + x] = proj_acc + A.proj_b;
-      asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-      __syncwarp();
-      if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar_tempty + 8 * a) : "memory");
+      wgmma_commit_wait();
+      // ---- epilogue: this thread's two pixels (h = 0, 1), one at a time ---------------------------------------------------
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int p = blk * 64 + qd * 16 + (lane >> 2) + 8 * h, pg = p >> 3;
+        const bool valid = pg < kMsRows * G;
+        const int r = pg / G, g = pg - r * G;
+        const int y = valid ? c * kMsRows + r : 0, x = valid ? 8 * g + (p & 7) : 0;
+        MsTap tp[NRS > 0 ? NRS : 1];
+        const float* rs[NRS > 0 ? NRS : 1];
+        int rpl[NRS > 0 ? NRS : 1];
+#pragma unroll
+        for (int j = 0; j < NRS; ++j) {
+          tp[j] = ms_tap(A.r_H[j], A.r_W[j], A.r_up[j], y, x);
+          rpl[j] = A.r_H[j] * A.r_W[j];
+          rs[j] = reinterpret_cast<const float*>(A.rsrc[j]) + ((size_t)n * A.r_C[j] + (size_t)A.r_c0[j]) * (size_t)rpl[j];
+        }
+        float proj_acc = 0.f;
+#pragma unroll
+        for (int i = 0; i < NN / 8; ++i) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int ch = 8 * i + 2 * q + e;                                 // channels >= C: zero weights, zero tables -> harmless work
+            const uint4 t4 = lds128(tab + (uint32_t)ch * 16u);
+            float v = d[4 * i + 2 * h + e] + __uint_as_float(t4.x);
+#pragma unroll
+            for (int t = 0; t < NRS; ++t) {
+              if (ch < A.r_n[t]) {                                            // (resample-add paths cover channels [0, r_n): checked by the host)
+                const float* s_ = rs[t] + ch * rpl[t];
+                v += tp[t].w00 * __ldg(s_ + tp[t].o00) + tp[t].w01 * __ldg(s_ + tp[t].o01) + tp[t].w10 * __ldg(s_ + tp[t].o10) +
+                     tp[t].w11 * __ldg(s_ + tp[t].o11);
+              }
+            }
+            v = prelu_m1(v, __uint_as_float(t4.y));
+            if (PROJ) proj_acc = fmaf(__uint_as_float(t4.z), v, proj_acc);
+            else if (valid && ch < C) {
+              const size_t o = ((size_t)n * C + (size_t)ch) * plane + (size_t)y * W + x;
+              if (A.dst_f32) reinterpret_cast<float*>(A.dst)[o] = v;
+              else reinterpret_cast<uint16_t*>(A.dst)[o] = Pack<T>::bits(v);
+            }
+          }
+        }
+        if (PROJ) {
+          proj_acc += __shfl_xor_sync(0xffffffffu, proj_acc, 1);
+          proj_acc += __shfl_xor_sync(0xffffffffu, proj_acc, 2);
+          if (q == 0 && valid) reinterpret_cast<float*>(A.dst)[((size_t)n * H + y) * W + x] = proj_acc + A.proj_b;
+        }
+      }
     }
+    warpgroup_bar(wg);                                                      // the group's MMAs of this chunk have all completed
+    if (qd == 0 && lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar_empty + 8 * s) : "memory");
+  }
+}
+
+template <typename T, int NRS, bool PROJ>
+__device__ __forceinline__ void ms_consume_n(const MsArgs& A, uint32_t sbase, uint32_t STG, uint32_t tab, uint32_t bar_ready, uint32_t bar_empty,
+                                             int ra, int rb, int wg, int qd, int lane) {
+  switch (A.NN) {
+    case 16: ms_consume<T, NRS, PROJ, 16>(A, sbase, STG, tab, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
+    case 32: ms_consume<T, NRS, PROJ, 32>(A, sbase, STG, tab, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
+    case 48: ms_consume<T, NRS, PROJ, 48>(A, sbase, STG, tab, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
+    case 64: ms_consume<T, NRS, PROJ, 64>(A, sbase, STG, tab, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
+    default: ms_consume<T, NRS, PROJ, 80>(A, sbase, STG, tab, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
   }
 }
 
@@ -135,28 +172,19 @@ mix_stream_kernel(const __grid_constant__ MsArgs A, const __grid_constant__ CUte
   const uint32_t sbase = (smem_u32(smem_raw) + 127u) & ~127u;
   uint8_t* gbase = smem_raw + (sbase - smem_u32(smem_raw));
   const uint32_t STG = sbase + A.off_stage, BAR = sbase + A.off_bar;
-  // barriers: full[8] at +0, empty[8] at +64, tmem full[8] at +128, tmem empty[8] at +192, built[8] at +256; TMEM base slot at +320
-  const uint32_t bar_full = BAR, bar_empty = BAR + 64, bar_tfull = BAR + 128, bar_tempty = BAR + 192, bar_built = BAR + 256;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(gbase + A.off_bar + 320);
+  // barriers: full[8] at +0, empty[8] at +64, built[8] at +128
+  const uint32_t bar_full = BAR, bar_empty = BAR + 64, bar_built = BAR + 128;
   const uint32_t TAB = sbase + A.off_tab;                                 // float4 {bias, slope - 1, proj, 0} per channel (kMsMaxC)
   float* tab = reinterpret_cast<float*>(gbase + A.off_tab);
-  const int NS = A.n_stages, NN = A.NN, nb = A.nb;
+  const int NS = A.n_stages, NN = A.NN;
 
   if (tid == 0) {
     for (int i = 0; i < NS; ++i) {
       asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;\n" ::"r"(bar_full + 8 * i) : "memory");
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;\n" ::"r"(bar_empty + 8 * i) : "memory");
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar_empty + 8 * i), "r"(kMsGroups) : "memory");   // one per consumer warpgroup
       asm volatile("mbarrier.init.shared::cta.b64 [%0], 2;\n" ::"r"(bar_built + 8 * i) : "memory");      // the two builder warps
     }
-    for (int i = 0; i < A.n_acc; ++i) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;\n" ::"r"(bar_tfull + 8 * i) : "memory");
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar_tempty + 8 * i), "r"(4 * A.nb) : "memory");   // 4 warps per block
-    }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;\n" ::"r"(BAR + 320) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
   }
   // weights of every conv path -> K-major B operand [n group][k group][8 n][8 k], zero outside the path's cout slice / cin
   for (int i = 0; i < A.n_in; ++i) {
@@ -180,10 +208,7 @@ mix_stream_kernel(const __grid_constant__ MsArgs A, const __grid_constant__ CUte
   }
   for (int i = tid; i < kMsMaxC; i += kMsThreads) { tab[4 * i] = A.bias[i]; tab[4 * i + 1] = A.has_slope ? A.sm1[i] : 0.f; tab[4 * i + 2] = A.proj[i]; tab[4 * i + 3] = 0.f; }
   asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  const uint32_t tmem = *tmem_slot;
 
   const int ra = (int)((long long)blockIdx.x * A.total_chunks / gridDim.x), rb = (int)((long long)(blockIdx.x + 1) * A.total_chunks / gridDim.x);
 
@@ -192,44 +217,13 @@ mix_stream_kernel(const __grid_constant__ MsArgs A, const __grid_constant__ CUte
     if (lane == 0) {
       for (int idx = ra, k = 0; idx < rb; ++idx, ++k) {
         const int s = k % NS, n = idx / A.cpi, c = idx - n * A.cpi;
-        if (k >= NS) mbar_wait_a(bar_empty + 8 * s, ((uint32_t)(k / NS) - 1u) & 1u);      // the stage's previous MMAs completed
+        if (k >= NS) mbar_wait_a(bar_empty + 8 * s, ((uint32_t)(k / NS) - 1u) & 1u);      // every consumer is done with the stage
         const uint32_t bar = bar_full + 8 * s, st = STG + (uint32_t)s * (uint32_t)A.stage_bytes;
         mbar_expect_tx_a(bar, (uint32_t)A.tx_bytes);
         const int y0 = kMsRows * c - (A.k3 ? 1 : 0);                       // 3x3: one halo row above (and below: the box is 2 rows taller)
         tma_load_5d(st + (uint32_t)A.in_off[0], &tm0, bar, 0, 0, 0, y0, n);
         if (A.n_in > 1) tma_load_5d(st + (uint32_t)A.in_off[1], &tm1, bar, 0, 0, 0, y0, n);
         if (A.n_in > 2) tma_load_5d(st + (uint32_t)A.in_off[2], &tm2, bar, 0, 0, 0, y0, n);
-      }
-    }
-  } else if (warp == 1) {
-    // ---- MMA issuer ----------------------------------------------------------------------------------------------
-    if (lane == 0) {
-      const uint32_t idesc = (1u << 4) | (1u << 15) | ((uint32_t)(NN >> 3) << 17) | (8u << 24);
-      for (int idx = ra, k = 0; idx < rb; ++idx, ++k) {
-        const int s = k % NS, a = k % A.n_acc;
-        mbar_wait_a((A.k3 ? bar_built : bar_full) + 8 * s, (uint32_t)(k / NS) & 1u);
-        if (k >= A.n_acc) mbar_wait_a(bar_tempty + 8 * a, ((uint32_t)(k / A.n_acc) - 1u) & 1u);       // the epilogue drained this accumulator buffer
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-        const uint32_t st = STG + (uint32_t)s * (uint32_t)A.stage_bytes;
-        for (int blk = 0; blk < nb; ++blk) {
-          uint32_t first = 1;
-          for (int i = 0; i < A.n_in; ++i) {
-            const int taps = A.k3 ? 9 : 1;
-            for (int tap = 0; tap < taps; ++tap) {
-              // 3x3: tap (ky, kx) reads copy kx (x-1 / centre / x+1 = copies 1 / 0 / 2) ky tile rows down
-              const int ky = tap / 3, kx = tap - 3 * ky, cp = kx == 1 ? 0 : (kx == 0 ? 1 : 2);
-              const uint32_t abase = st + (uint32_t)A.in_off[i] + (A.k3 ? (uint32_t)cp * (uint32_t)A.copy_bytes[i] + (uint32_t)(ky * A.G * A.S[i]) * 16u : 0u);
-              const uint64_t da = umma_desc(abase + (uint32_t)(blk * 16 * A.S[i]) * 16u, 128u, (uint32_t)A.S[i] * 16u);
-              const uint64_t db = umma_desc(sbase + (uint32_t)A.off_wb[i] + (uint32_t)(tap * NN * A.K16[i] * 2), 128u, (uint32_t)(A.K16[i] >> 3) * 128u);
-              for (int ks = 0; ks < (A.K16[i] >> 4); ++ks) {
-                umma_f16(tmem + (uint32_t)(a * nb * NN + blk * NN), da + (uint64_t)(16 * ks), db + (uint64_t)(16 * ks), idesc, first ^ 1u);
-                first = 0;
-              }
-            }
-          }
-        }
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar_empty + 8 * s) : "memory");
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar_tfull + 8 * a) : "memory");
       }
     }
   } else if (warp == 2 || warp == 3) {
@@ -260,17 +254,13 @@ mix_stream_kernel(const __grid_constant__ MsArgs A, const __grid_constant__ CUte
       }
     }
   } else if (warp >= 4) {
-    // ---- epilogue: a group of 4 warps (one per TMEM lane quarter) takes the (chunk, block) tasks t = k * nb + blk with
-    //      t % groups == its index, so several chunks are drained concurrently ---------------------------------------------
-    const int e = warp - 4, q = e & 3, grp = e >> 2;
-    if (A.has_proj) ms_epilogue<T, 0, true>(A, tmem, TAB, bar_tfull, bar_tempty, ra, rb, q, grp, lane);
-    else if (A.n_rs == 0) ms_epilogue<T, 0, false>(A, tmem, TAB, bar_tfull, bar_tempty, ra, rb, q, grp, lane);
-    else if (A.n_rs == 1) ms_epilogue<T, 1, false>(A, tmem, TAB, bar_tfull, bar_tempty, ra, rb, q, grp, lane);
-    else ms_epilogue<T, 2, false>(A, tmem, TAB, bar_tfull, bar_tempty, ra, rb, q, grp, lane);
+    const int e = warp - 4, qd = e & 3, wg = e >> 2;
+    const uint32_t ready = A.k3 ? bar_built : bar_full;
+    if (A.has_proj) ms_consume_n<T, 0, true>(A, sbase, STG, TAB, ready, bar_empty, ra, rb, wg, qd, lane);
+    else if (A.n_rs == 0) ms_consume_n<T, 0, false>(A, sbase, STG, TAB, ready, bar_empty, ra, rb, wg, qd, lane);
+    else if (A.n_rs == 1) ms_consume_n<T, 1, false>(A, sbase, STG, TAB, ready, bar_empty, ra, rb, wg, qd, lane);
+    else ms_consume_n<T, 2, false>(A, sbase, STG, TAB, ready, bar_empty, ra, rb, wg, qd, lane);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;\n" ::"r"(tmem) : "memory");
 }
 
 }  // namespace csnet

@@ -199,7 +199,7 @@ struct csnet_plan {
   std::vector<char> op_ms;                        // per op: the streaming 1x1 MIX kernel (mix_stream.cuh) can run it
   bool ms_enabled = true;                         // CSNET_MS=0 at plan creation: mix_tc / generic kernels only
   std::vector<char> op_ils;                       // per op: the streaming ILBlock kernel (il_stream.cuh) can run it
-  int num_sms = 148;
+  int num_sms = 132;
   int ils_force_ns = 0;                           // CSNET_ILS_NS=k: force k column strips (0: automatic)
   bool ils_enabled = true;                        // CSNET_ILS=0 at plan creation: tiled kernel only
   int ils_min_chunks = 592;                       // batches with fewer 4-row chunks per ILBlock run the tiled kernel
@@ -497,7 +497,7 @@ bool encode_image_map(CUtensorMap* tm, const void* base, int N, int C, int H, in
 }
 
 // Geometry of the streaming ILBlock kernel for an op; false if the op does not qualify (the tiled kernel runs it).
-// Picks the column-strip split: the fewest strips that fit the thread / shared-memory / TMEM limits.
+// Picks the column-strip split: the fewest strips that fit the thread / shared-memory limits.
 bool make_ils(const csnet_plan& P, const csnet_op_desc& op, csnet::IlsArgs* out) {
   if (!P.ils_enabled || op.kind != CSNET_OP_ILBLOCK || encode_tiled_fn() == nullptr) return false;
   const csnet_tensor_desc &Xh = P.tensors[op.paths[0].src], &Xl = P.tensors[op.paths[1].src], &Yh = P.tensors[op.dst];
@@ -529,14 +529,10 @@ bool make_ils(const csnet_plan& P, const csnet_op_desc& op, csnet::IlsArgs* out)
     T.ns = ns; T.gsn = A.GH / ns; T.hl = ns > 1 ? 1 : 0;
     T.GR = T.gsn + 2 * T.hl; T.GLR = T.gsn / 2 + 2 * T.hl;
     T.dw_warps = (T.Cho * T.gsn + T.Clo * (T.gsn / 2) + 31) / 32;        // tail tasks are packed: hi (channel, column)s, then lo ones
-    if (T.dw_warps < 4) T.dw_warps = 4;                                   // the epilogue needs one warp per TMEM lane quarter
+    if (T.dw_warps < 4) T.dw_warps = 4;                                   // the GEMM needs one warpgroup
     const int warps = T.dw_warps;
     if (warps * 32 > csnet::kIlsMaxThreads || T.SH > 256 || T.SL > 256 || T.GR > 256) continue;
-    const int nbh = (4 * T.GR + 15) / 16, nbl = T.Clo > 0 ? (2 * T.GLR + 15) / 16 : 0;
-    const int cols = nbh * T.NH + nbl * T.NL;                              // fp32 accumulators of a chunk: TMEM columns
-    if (cols > 512 || nbh + nbl > 16) continue;
-    T.tmem_cols = 32;
-    while (T.tmem_cols < cols) T.tmem_cols *= 2;
+    const int nbh = (4 * T.GR + 7) / 8, nbl = T.Clo > 0 ? (2 * T.GLR + 7) / 8 : 0;     // 64-pixel GEMM blocks of a chunk
     T.BW = 8 * T.GR + 8;                                                  // stem: image block row = the tile's pixels + 4 on each side
     if (stem && T.BW > 256) continue;
     T.lo_stage_bytes = stem ? r128(T.BW * 4 * T.Ci * 4) : r128(2 * T.GLR * T.SL * 16);
@@ -551,16 +547,14 @@ bool make_ils(const csnet_plan& P, const csnet_op_desc& op, csnet::IlsArgs* out)
     T.off_epi = T.off_zero + 128;                          // 4 tables of 64 floats + 512 bytes of scratch rows
     T.off_xlo = T.off_epi + 1536;                          // stem: GEMM operand of the lo chunk (the ring holds image blocks)
     int end = T.off_xlo + (stem ? r128(2 * T.GLR * T.SL * 16) : 0);
-    // the last accumulator block of a chunk reads (never uses) up to 15 pixel groups past the chunk: keep them inside
-    const int over_h = T.off_xh + T.hi_stage_bytes + nbh * 16 * T.SH * 16,
-              over_l = (stem ? T.off_xlo : T.off_xl + 2 * T.lo_stage_bytes) + nbl * 16 * T.SL * 16;
+    // the last GEMM block of a chunk reads (never uses) up to 7 pixel groups past the chunk: keep them inside
+    const int over_h = T.off_xh + T.hi_stage_bytes + nbh * 8 * T.SH * 16,
+              over_l = (stem ? T.off_xlo : T.off_xl + 2 * T.lo_stage_bytes) + nbl * 8 * T.SL * 16;
     end = over_h > end ? over_h : end;
     end = over_l > end ? over_l : end;
     T.smem_bytes = end + 128;
     if (T.smem_bytes > 227 * 1024) continue;
     // cost model: the depthwise tail (~55 % of a chunk) does not see the halo groups, everything else scales with them.
-    // (Narrow strips do NOT buy a second CTA per SM: a kernel that touches tcgen05 is resident once per SM — measured with
-    // scripts/occ_probe.cu: occupancy 1 for any kernel with tcgen05.alloc / commit, whatever its shared memory.)
     const double cost = 0.55 + 0.45 * T.GR / T.gsn;
     if (!found || cost < best_cost) { best = T; best_cost = cost; found = true; }
   }
@@ -637,10 +631,7 @@ bool make_ms(const csnet_plan& P, const csnet_op_desc& op, int N, const void* co
   A.stage_bytes = off;
   A.tx_bytes = 0;
   for (int i = 0; i < A.n_in; ++i) A.tx_bytes += (csnet::kMsRows + (A.k3 ? 2 : 0)) * A.G * A.S[i] * 16;
-  A.nb = (csnet::kMsRows * A.G + 15) / 16;
-  A.n_acc = 512 / (A.nb * A.NN);
-  A.n_acc = A.n_acc > 8 ? 8 : A.n_acc;
-  if (A.n_acc < 2) return false;
+  A.nb = (csnet::kMsRows * A.G + 7) / 8;
   A.cpi = D.H / csnet::kMsRows;
   A.total_chunks = N * A.cpi;
   int wb = 0;
@@ -970,7 +961,7 @@ static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_
       csnet::msd_launch<__half>(q.dil, A, stream);
     }
   } else if (P->op_ms[i] && (int64_t)P->max_batch * (D.H / csnet::kMsRows) >= (int64_t)2 * P->num_sms) {
-    // streaming 1x1 MIX kernel (mix_stream.cuh): TMA operand tiles -> tcgen05 -> epilogue (resample-adds, PReLU, projection)
+    // streaming 1x1 MIX kernel (mix_stream.cuh): TMA operand tiles -> wgmma -> epilogue (resample-adds, PReLU, projection)
     csnet::MsArgs A;
     CUtensorMap maps[csnet::kMsMaxIn];
     memset(maps, 0, sizeof maps);
@@ -1028,7 +1019,7 @@ static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_
     gn_apply_kernel<<<dim3(bx < 1 ? 1 : bx, D.C, N), kThreads, 0, stream>>>(A);
   } else if (op.kind == CSNET_OP_ILBLOCK && P->op_ils[i] && (int64_t)P->max_batch * (D.H / 4) >= (int64_t)P->ils_min_chunks) {
     // (the choice depends on the plan's max_batch, not on N: every sub-batch of a plan runs the same kernels, bit for bit)
-    // streaming kernel (il_stream.cuh): TMA operand tiles, tcgen05 GEMM, register-resident depthwise tail
+    // streaming kernel (il_stream.cuh): TMA operand tiles, wgmma GEMM, register-resident depthwise tail
     csnet::IlsArgs A;
     if (!make_ils(*P, op, &A)) return fail(CSNET_E_UNSUPPORTED, "ILBLOCK op no longer qualifies for the streaming kernel");
     auto f = [&](int e) { return op.ext_off[e] >= 0 ? P->blob + op.ext_off[e] : nullptr; };
@@ -1066,7 +1057,7 @@ static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_
       for (int b = 0; b < grid; ++b) for (int k = 0; k < 8; ++k) m[k] += (double)h[(size_t)b * 8 + k] / grid;
       int occ = -1;
       cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, csnet::il_stream_kernel<__half, true>, A.dw_warps * 32, A.smem_bytes);
-      fprintf(stderr, "[ils ns %d grid %d threads %d smem %d tmem %d occupancy %d] ", A.ns, grid, A.dw_warps * 32, A.smem_bytes, A.tmem_cols, occ);
+      fprintf(stderr, "[ils ns %d grid %d threads %d smem %d occupancy %d] ", A.ns, grid, A.dw_warps * 32, A.smem_bytes, occ);
       fprintf(stderr, "[ils %dx%d C %d+%d->%d+%d] cycles/CTA: load-wait %.0f resample %.0f syncA %.0f issue %.0f epilogue %.0f syncB %.0f dw %.0f tail %.0f\n",
               A.H, A.W, A.Chi, A.Cli, A.Cho, A.Clo, m[0], m[1], m[2], m[3], m[4], m[5], m[6], m[7]);
     }
@@ -1218,14 +1209,14 @@ const char* csnet_plan_op_kernel(const csnet_plan* P, int32_t i) {
   const csnet_op_desc& op = P->ops[i];
   const csnet_tensor_desc& D = P->tensors[op.dst];
   if (P->op_msd[i]) return "msd_kernel (ms_direct.cuh, FP32 pipe)";
-  if (P->op_ms[i] && (int64_t)P->max_batch * (D.H / csnet::kMsRows) >= (int64_t)2 * P->num_sms) return "mix_stream_kernel (TMA + tcgen05)";
+  if (P->op_ms[i] && (int64_t)P->max_batch * (D.H / csnet::kMsRows) >= (int64_t)2 * P->num_sms) return "mix_stream_kernel (TMA + wgmma)";
   if ((op.kind == CSNET_OP_MIX || op.kind == CSNET_OP_MIXPROJ) && P->op_tc[i].mt > 0) return "mix_tc_kernel (mma.sync)";
   if (op.kind == CSNET_OP_MIX && op.n_paths == 1 && op.paths[0].ksize == 0 && op.paths[0].cout0 == 0 && op.paths[0].cout == D.C)
     return "pool2 / upsample / resample kernels";
   if (op.kind == CSNET_OP_MIX) return "mix_generic_kernel";
   if (op.kind == CSNET_OP_GN) return "gn kernels";
   if (op.kind == CSNET_OP_ILBLOCK && P->op_ils[i] && (int64_t)P->max_batch * (D.H / 4) >= (int64_t)P->ils_min_chunks)
-    return "il_stream_kernel (TMA + tcgen05 + TMEM)";
+    return "il_stream_kernel (TMA + wgmma)";
   if (op.kind == CSNET_OP_ILBLOCK) return "il_block_kernel (mma.sync, tiled)";
   return "dw kernels";
 }

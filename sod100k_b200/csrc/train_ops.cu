@@ -47,7 +47,7 @@ __device__ __forceinline__ void block_sum3(float& a, float& b, float& c) {
 }
 
 // ---- BatchNorm (train) + PReLU ---------------------------------------------------------------------------
-// Per-channel reductions over (N, H*W) run on a (C, parts) grid — a channel-per-block grid would leave most of the 148 SMs
+// Per-channel reductions over (N, H*W) run on a (C, parts) grid — a channel-per-block grid would leave most of the 132 SMs
 // idle for 8..79-channel layers.  A block reduces one segment of one image plane, publishes its partial to a workspace,
 // and the last block to arrive for a channel (ticket counter) merges the partials IN PART ORDER, so the result does not
 // depend on scheduling.  Segments: S per plane, parts = N * S.
@@ -555,9 +555,9 @@ static int num_sms() {
   static int sms[kMaxDevices] = {0};
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 0 || dev >= kMaxDevices) return 148;
+  if (dev < 0 || dev >= kMaxDevices) return 132;
   if (!sms[dev]) cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
-  return sms[dev] > 0 ? sms[dev] : 148;
+  return sms[dev] > 0 ? sms[dev] : 132;
 }
 
 static bool conv_tile_geometry(tf::ConvArgs& A) {

@@ -106,7 +106,7 @@ class ModelEngine:
         if x.dim() != 4 or x.shape[1] != 3:
             raise ValueError(f"expected input [N,3,H,W], got {tuple(x.shape)}")
         if not x.is_cuda:
-            raise runtime.EngineError("CSNet (B200 engine) needs a CUDA input; call model.cuda() / input.cuda() "
+            raise runtime.EngineError("CSNet (CUDA engine) needs a CUDA input; call model.cuda() / input.cuda() "
                                       "as the reference's test.py does — there is no CPU path")
         if self.model.training:
             from . import modular

@@ -1,9 +1,9 @@
-"""`model.csnet` — the reference's module surface on the B200 engine.
+"""`model.csnet` — the reference's module surface on the CUDA engine.
 
 Same class names, constructor arguments, parameter names, buffers and `state_dict()` keys as
 /root/reference/CSNet/model/csnet.py (SURVEY.md §8b), so `test.py` / `train.py` / checkpoints work
 unchanged — but the modules here are PARAMETER CONTAINERS: `CSNet.forward` lowers the whole network to one
-program of fused sm_100a kernels (sod100k_b200/compiler.py -> libcsnet_b200.so) instead of calling
+program of fused sm_90a kernels (sod100k_b200/compiler.py -> libcsnet_b200.so) instead of calling
 torch.nn.functional per layer.  There is no torch/cuDNN fallback: without the library or a GPU it raises.
 
 Construction order and initialisers follow the reference (conv weights `kaiming_uniform_(a=sqrt(5))`,

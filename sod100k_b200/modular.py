@@ -150,7 +150,7 @@ def ms_block_forward(m, x):
 def csnet_forward(model, x):
     """CSNet.forward (csnet.py:365-387) on the module-granular kernels."""
     if not x.is_cuda:
-        raise T.runtime.EngineError("CSNet (B200 engine) needs CUDA tensors; there is no CPU path")
+        raise T.runtime.EngineError("CSNet (CUDA engine) needs CUDA tensors; there is no CPU path")
     if x.shape[2] % 16 or x.shape[3] % 16:
         raise ValueError(f"input size {tuple(x.shape[2:])} must be a multiple of 16")
     feats, cur = {}, [x.float()]

@@ -1,4 +1,4 @@
-"""`networks.csf_res2net` — the reference's CSF+Res2Net module surface (config 5) on the B200 engine.
+"""`networks.csf_res2net` — the reference's CSF+Res2Net module surface (config 5) on the CUDA engine.
 
 Same class / parameter names and `state_dict()` keys as /root/reference/CSF+Res2Net/networks/{csf_res2net,gOctConv}.py
 so `solver.py` (`build_model()`, `net.base.load_pretrained_model`, `load_state_dict(strict=False)`) keeps working.
@@ -198,7 +198,7 @@ class CSFNet(nn.Module):
 
     def forward(self, x):
         if not x.is_cuda:
-            raise runtime.EngineError("CSFNet (B200 engine) needs CUDA tensors; there is no CPU path")
+            raise runtime.EngineError("CSFNet (CUDA engine) needs CUDA tensors; there is no CPU path")
         if self.training or torch.is_grad_enabled():
             raise NotImplementedError("CSF+Res2Net runs inference only (config 5): call under model.eval() and torch.no_grad()")
         n, _, h, w = x.shape

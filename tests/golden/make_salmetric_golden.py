@@ -59,7 +59,7 @@ if __name__ == "__main__":
 
     binary = build_ref.build()
     cases = {}
-    for name, (seed, n, h, w) in {"a": (11, 5, 24, 32), "b": (12, 3, 40, 40), "c": (13, 7, 16, 48)}.items():
+    for name, (seed, n, h, w) in {"a": (11, 5, 24, 32), "b": (12, 3, 40, 40), "c": (13, 7, 16, 48), "d": (21, 6, 20, 28)}.items():
         sal, gt = seeded_maps(seed, n, h, w)
         cases[name] = {"args": [seed, n, h, w], "report": run_reference(binary, sal, gt)}
     json.dump(cases, open(os.path.join(HERE, "salmetric_ref.json"), "w"), indent=1)

@@ -1,4 +1,4 @@
-"""The streaming ILBlock kernel (csrc/il_stream.cuh: TMA operand tiles, tcgen05 GEMM with TMEM accumulators, register-resident
+"""The streaming ILBlock kernel (csrc/il_stream.cuh: TMA operand tiles, wgmma GEMM with register accumulators, register-resident
 depthwise tail) against the generic ops, the tiled kernel and the oracle.  CSNET_ILS / CSNET_ILS_MIN_CHUNKS / CSNET_ILS_NS are
 read when a plan is created, so a test can pin which kernel runs an ILBLOCK op."""
 import os
@@ -89,7 +89,7 @@ def test_streaming_kernel_is_deterministic_and_batch_independent():
 
 @pytest.mark.parametrize("tag,hw,nb", [("csnet-L-x2", (224, 224), 24), ("csnet-L-x1", (224, 224), 24), ("csnet-L-x2", (96, 160), 40)])
 def test_streaming_mix_kernel_matches_the_tensor_core_mix_kernel(tag, hw, nb):
-    """csrc/mix_stream.cuh (TMA -> tcgen05 -> epilogue with resample-adds / the cls_layer projection) on and off for the same
+    """csrc/mix_stream.cuh (TMA -> wgmma -> epilogue with resample-adds / the cls_layer projection) on and off for the same
     fp16 program: taps of the CSF head and the logits.  Both sides run fp16 operands with fp32 accumulation; the differences are
     accumulation order and the 16-bit rounding of the stored taps."""
     cfg, sd = fixtures.checkpoint(tag)

@@ -82,8 +82,7 @@ def test_forward_backward_matches_oracle(tag, hw, n):
     # DISCRETE decision taken differently by two fp32 implementations — a max-pool arg-max or a PReLU sign at a near-tie, reached
     # through a 1-ulp difference upstream: the gradient is then a different (equally valid) sub-gradient, off by 0.5-2 % on the
     # small tensors of stage 4, while the fp32 and float64 oracles (same summation order) still agree to 1e-5.  scripts/grad_diag.py
-    # (profiles/r02_i_grad_diag.md) shows it: same input size, seeds 52 / 53 -> 162 / 383 tensors above 5e-4 with the round-1
-    # kernels, the round-2 kernels and either BatchNorm-statistics kernel alike, seed 53 clean again with the two-pass statistics.
+    # shows such flips per tensor.
     # The pruned x1 checkpoint sits on such kinks in most runs, so it keeps the global L2 bound + 5e-2 per-tensor cap.
     _check_grads(m, ref_grads, _oracle_fp64_grads(cfg, params, buffers, x, t), floor=GRAD_TOL if tag == "csnet-L-x2" else 2 * GRAD_TOL,
                  per_tensor=tag != "csnet-L-x1")
