@@ -189,7 +189,8 @@ void csnet_plan_destroy(csnet_plan* plan);
  * Convenience for hosts that keep their data in pageable/pinned HOST memory (the e2e path of
  * bench.py and of CSNet/test.py:86-93): copies x (fp32 NCHW, N*3*H*W floats) to the device, runs,
  * copies the logits (N*H*W floats) back and returns when y_host is complete.  Batches of 64 or more are cut into
- * four chunks that pipeline H2D copy / kernels / D2H copy on separate streams (use pinned host memory).
+ * three chunks (N/8, the rest, N/8) that pipeline H2D copy / kernels / D2H copy on separate streams (use pinned host memory).
+ * Smaller batches, and every batch of csnet_plan_run_host_u8, run as one chunk.
  * The plan must bind external 0 = input, external 1 = logits.
  */
 int csnet_plan_run_host(csnet_plan* plan, int32_t N, const float* x_host, float* y_host, void* stream);

@@ -1,4 +1,4 @@
-"""Per-op times of the fp16 bs-256 program (streaming ILBlock kernel on); CSNET_ILS_DBG=1 prints the phase cycle counters."""
+"""Per-op times of the fp16 bs-256 program (streaming ILBlock kernel on)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

@@ -29,6 +29,8 @@
 // warm-up chunk where a CTA's range starts inside an image); the work split is a flat division of the
 // N * ns * H/4 chunks over the CTAs.  Needs W % 16 == 0, H % 4 == 0, K = Chi + Cli <= 64.  Other shapes: il_block.cuh.
 #pragma once
+#include <cuda.h>
+
 #include "il_block.cuh"
 
 namespace csnet {
@@ -56,7 +58,6 @@ struct IlsArgs {
   int32_t cpi, total_chunks;          // chunks per image strip (H/4), N * ns * cpi
   int32_t dw_warps;                   // warps of the CTA = warps of the depthwise tail (tasks packed: hi columns, then lo)
   int32_t hi_stage_bytes, lo_stage_bytes;
-  unsigned long long* dbg;             // optional: per-CTA phase cycle counters [grid][8] (CSNET_ILS_DBG=1)
   int32_t off_xl, off_xh, off_t1l, off_wbh, off_wbl, off_bar, off_zero, off_epi, smem_bytes;
 };
 
@@ -265,7 +266,7 @@ __device__ __forceinline__ void ils_block_n(int N, uint64_t da, uint64_t db, int
   }
 }
 
-template <typename T, bool kTiming = false, bool kStem = false>
+template <typename T, bool kStem = false>
 __global__ void __launch_bounds__(kIlsMaxThreads, 1)
 il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUtensorMap tmH, const __grid_constant__ CUtensorMap tmL) {
   extern __shared__ uint8_t smem_raw[];
@@ -366,9 +367,6 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
   int ra = (int)((long long)blockIdx.x * A.total_chunks / gridDim.x);
   const int rb = (int)((long long)(blockIdx.x + 1) * A.total_chunks / gridDim.x);
   uint32_t hq = 0, lq = 0;                               // running counts: hi loads, lo loads
-  long long tph[8] = {0, 0, 0, 0, 0, 0, 0, 0}, tlast = clock64();
-  const bool timing = kTiming && A.dbg != nullptr && tid == 0;
-#define ILS_MARK(i) do { if (kTiming && timing) { const long long t_ = clock64(); tph[i] += t_ - tlast; tlast = t_; } } while (0)
 
   while (ra < rb) {
     const int item = ra / cpi, ca = ra - item * cpi;
@@ -425,7 +423,6 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
           ++lo_waited;
         }
       }
-      ILS_MARK(0);
       const uint32_t xh = hi_stage(c), xl = kStem ? XLO : lo_stage(c);
       if (kStem) {
         // ---- 2s. im2col of the image chunk (hi) and of its 2x2 max-pool (lo): a task = one (row, group, ci, ky) and makes
@@ -549,17 +546,14 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
           }
         }
       }
-      ILS_MARK(1);
       asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");    // generic writes -> visible to the tensor core / TMA
       __syncthreads();                                                    // (A)
-      ILS_MARK(2);
       // ---- 3. next loads (one thread of the last warp) ------------------------------------------------------
       if (warp == nwarps - 1 && lane == 0) {
         asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
         if (!kStem && c >= c0 + 1 && c + 1 <= c1) issue_hi(c + 1);       // stage of chunk c-1: its T1 was consumed
         if (c + 2 <= cl1) issue_lo(c + 2);                               // stage of lo chunk c-1: last read by this chunk's up-sample
       }
-      ILS_MARK(3);
       // ---- 4. GEMM + epilogue: warpgroup w takes the 64-pixel blocks w, w + wgs, ..; fp32 accumulators in registers ->
       //         bias, PReLU, 16-bit -> T1 (hi: in place over the block's own pixel groups; lo: its own buffer) ----------------
       if (warp < (nwarps & ~3)) {
@@ -573,9 +567,7 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
                            (uint32_t)ST * 16u, (b - nbh) * 8 + qd * 2, 2 * GLR, EPI + 512u, EPI + 768u, DUMMY, lane);
         }
       }
-      ILS_MARK(4);
       __syncthreads();                                                    // (B)
-      ILS_MARK(5);
       // ---- 5. depthwise tail over the chunk's rows --------------------------------------------------------
       if (dw_live) {
         const uint32_t t1b = (dw_hi ? xh : T1L) + dw_off;
@@ -593,7 +585,6 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
           ils_dw_push<T>(t1w, t2w, n1, w1, b1, s1, w2, b2, s2, make_t2, mL, mR, make_out, ybase + (size_t)orow * dWd);
         }
       }
-      ILS_MARK(6);
     }
     // ---- image bottom: two rows of zero padding flush the last two output rows ----------------------------
     if (cb == cpi && dw_live) {
@@ -605,12 +596,6 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
     }
     __syncthreads();          // every shared-memory read of this piece is done before the next piece's loads overwrite it
   }
-
-  if (timing) {
-    ILS_MARK(7);
-    for (int i = 0; i < 8; ++i) A.dbg[(size_t)blockIdx.x * 8 + i] = (unsigned long long)tph[i];
-  }
-#undef ILS_MARK
 }
 
 }  // namespace csnet

@@ -170,6 +170,12 @@ struct TcChoice {
   int kk = 1;            // largest tap count among the conv paths
 };
 
+// The kernel (family) launch_op() runs for an op, chosen once per op when the plan is created (choose_kernel).
+enum class Kern : uint8_t { Msd, MixStream, MixTc, Pool2, Upsample, Resample, MixGeneric, Gn, IlStream, IlBlock, DwFast, DwGeneric };
+
+// Small batches of a two-external plan up to this size replay a captured graph (csnet_plan_run).
+constexpr int kGraphMaxN = 8;
+
 size_t tc_smem_bytes(const TcChoice& c) {
   return ((size_t)c.kc * c.xs_halves + (size_t)c.kk * c.mt * 16 * (c.kc + 8)) * 2;
 }
@@ -194,11 +200,8 @@ struct csnet_plan {
   struct GraphSlot { cudaGraphExec_t exec = nullptr; void* in = nullptr; void* out = nullptr; size_t in_bytes = 0, out_bytes = 0; };
   std::vector<GraphSlot> graphs;                  // index = batch size
   cudaStream_t cap_stream = nullptr;
-  int graph_max_n = 8;                            // CSNET_GRAPH_MAX_N (0 disables)
-  std::vector<char> op_msd;                       // per op: an MSBlock whose dilated paths run on ms_direct.cuh
-  std::vector<char> op_ms;                        // per op: the streaming 1x1 MIX kernel (mix_stream.cuh) can run it
+  std::vector<Kern> op_kern;                      // per op: the kernel launch_op() runs
   bool ms_enabled = true;                         // CSNET_MS=0 at plan creation: mix_tc / generic kernels only
-  std::vector<char> op_ils;                       // per op: the streaming ILBlock kernel (il_stream.cuh) can run it
   int num_sms = 132;
   int ils_force_ns = 0;                           // CSNET_ILS_NS=k: force k column strips (0: automatic)
   bool ils_enabled = true;                        // CSNET_ILS=0 at plan creation: tiled kernel only
@@ -403,20 +406,6 @@ EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
-// 4-D map over a planar [N][C][H][W] 16-bit tensor, box = (bw, bh, bc, 1) -> dense [bc][bh][bw] in shared memory,
-// out-of-bounds elements read as zero (the conv zero padding / "outside the image" of the fused kernels).
-bool encode_plane_map(CUtensorMap* tm, const void* base, int N, int C, int H, int W, int bw, int bh, int bc) {
-  EncodeTiledFn fn = encode_tiled_fn();
-  if (!fn) return false;
-  const cuuint64_t dims[4] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)C, (cuuint64_t)N};
-  const cuuint64_t strides[3] = {(cuuint64_t)W * 2, (cuuint64_t)H * W * 2, (cuuint64_t)C * H * W * 2};
-  const cuuint32_t box[4] = {(cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bc, 1};
-  const cuuint32_t estr[4] = {1, 1, 1, 1};
-  return fn(tm, CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<void*>(base), dims, strides, box, estr,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 // Fill the kernel arguments of a fused ILBlock op and pick its tile; false if no tile fits shared memory.
 bool make_il(const csnet_plan& P, const csnet_op_desc& op, int N, const void* const* ext, csnet::IlArgs* out) {
   csnet::IlArgs A{};
@@ -441,9 +430,6 @@ bool make_il(const csnet_plan& P, const csnet_op_desc& op, int N, const void* co
   A.ML16 = A.Clo > 0 ? round_up(A.Clo, 16) : 0;
   A.rowsAh = A.K8 > A.Cho ? A.K8 : A.Cho;
   A.rowsAl = A.Clo > 0 ? (A.K8 > A.Clo ? A.K8 : A.Clo) : A.Cli;
-  static const bool use_tma = [] { const char* e = getenv("CSNET_TMA"); return e && e[0] == '1'; }();   // opt-in until the 16-byte start-alignment rule is met (see DESIGN.md)
-  A.tma_h = use_tma && !A.first && (A.W % 8 == 0) && encode_tiled_fn() != nullptr;
-  A.tma_l = use_tma && !A.first && ((A.W / 2) % 8 == 0) && encode_tiled_fn() != nullptr;
   static const int cand[][2] = {{32, 32}, {28, 32}, {16, 64}, {16, 32}, {8, 16}};   // the instantiated tile geometries
   double best = -1;
   for (int chunked = 0; chunked < 2; ++chunked) {
@@ -572,8 +558,7 @@ bool make_ils(const csnet_plan& P, const csnet_op_desc& op, csnet::IlsArgs* out)
 // MSBlock form of a MIX op: every path a dilated 3x3 (pad == dil in {1, 2, 4, 8, 16}, stride 1) of the SAME whole fp16 tensor,
 // at most 8 output channels per path (the concat = disjoint cout slices), fp16 destination of the same size.
 bool is_msd(const csnet_plan& P, const csnet_op_desc& op) {
-  static const bool enabled = [] { const char* e = getenv("CSNET_MSD"); return !(e && e[0] == '0'); }();
-  if (!enabled || op.kind != CSNET_OP_MIX || op.ext_off[23] == 1 || op.n_paths < 1) return false;
+  if (op.kind != CSNET_OP_MIX || op.ext_off[23] == 1 || op.n_paths < 1) return false;
   const csnet_tensor_desc& D = P.tensors[op.dst];
   if (D.dtype != CSNET_F16 || D.W % 8) return false;
   for (int p = 0; p < op.n_paths; ++p) {
@@ -662,12 +647,12 @@ bool make_ms(const csnet_plan& P, const csnet_op_desc& op, int N, const void* co
 }
 
 template <typename T>
-void launch_il_t(const csnet::IlArgs& A, dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& h, const CUtensorMap& l) {
-  if (A.TH == 32) csnet::il_block_kernel<T, 32, 32><<<grid, csnet::kIlThreads, smem, st>>>(A, h, l);
-  else if (A.TH == 28) csnet::il_block_kernel<T, 28, 32><<<grid, csnet::kIlThreads, smem, st>>>(A, h, l);
-  else if (A.TH == 16 && A.TW == 64) csnet::il_block_kernel<T, 16, 64><<<grid, csnet::kIlThreads, smem, st>>>(A, h, l);
-  else if (A.TH == 16) csnet::il_block_kernel<T, 16, 32><<<grid, csnet::kIlThreads, smem, st>>>(A, h, l);
-  else csnet::il_block_kernel<T, 8, 16><<<grid, csnet::kIlThreads, smem, st>>>(A, h, l);
+void launch_il_t(const csnet::IlArgs& A, dim3 grid, size_t smem, cudaStream_t st) {
+  if (A.TH == 32) csnet::il_block_kernel<T, 32, 32><<<grid, csnet::kIlThreads, smem, st>>>(A);
+  else if (A.TH == 28) csnet::il_block_kernel<T, 28, 32><<<grid, csnet::kIlThreads, smem, st>>>(A);
+  else if (A.TH == 16 && A.TW == 64) csnet::il_block_kernel<T, 16, 64><<<grid, csnet::kIlThreads, smem, st>>>(A);
+  else if (A.TH == 16) csnet::il_block_kernel<T, 16, 32><<<grid, csnet::kIlThreads, smem, st>>>(A);
+  else csnet::il_block_kernel<T, 8, 16><<<grid, csnet::kIlThreads, smem, st>>>(A);
 }
 
 template <typename T>
@@ -684,9 +669,8 @@ cudaError_t set_il_smem_t(int bytes) {
 // paths and at most 80 output channels; ext_off[23] == 1 is the compiler's veto (weights overflow 16 bits).
 TcChoice choose_tc(const csnet_plan& P, const csnet_op_desc& op) {
   TcChoice c;
-  static const bool enabled = [] { const char* e = getenv("CSNET_TC"); return !(e && e[0] == '0'); }();
   if (op.kind == CSNET_OP_MIXPROJ) { /* no other kernel implements it */ }
-  else if (!enabled || op.kind != CSNET_OP_MIX || op.ext_off[23] == 1) return c;
+  else if (op.kind != CSNET_OP_MIX || op.ext_off[23] == 1) return c;
   const csnet_tensor_desc& D = P.tensors[op.dst];
   const int Cm = mix_channels(P, op);
   int dt = D.dtype != CSNET_F32 ? D.dtype : -1, pad = 0, nconv = 0, kk = 1, cin_max = 0;
@@ -715,6 +699,35 @@ TcChoice choose_tc(const csnet_plan& P, const csnet_op_desc& op) {
     if (kc <= ((cin_max + 7) & ~7) && tc_smem_bytes(t) <= 100 * 1024) { c.kc = kc; break; }
   }
   return c;
+}
+
+// The kernel that runs op i; the first one in this order that takes the op wins.  Every input is fixed when the plan is
+// created (the op, its tensors, op_tc, max_batch, the SM count, the switches), never by the batch of a call: every sub-batch
+// of a plan runs the same kernels, bit for bit.
+Kern choose_kernel(const csnet_plan& P, size_t i) {
+  const csnet_op_desc& op = P.ops[i];
+  const csnet_tensor_desc& D = P.tensors[op.dst];
+  csnet::MsArgs M;
+  csnet::IlsArgs S;
+  if (is_msd(P, op)) return Kern::Msd;
+  if (make_ms(P, op, 1, nullptr, &M, nullptr) && (int64_t)P.max_batch * (D.H / csnet::kMsRows) >= (int64_t)2 * P.num_sms)
+    return Kern::MixStream;
+  if ((op.kind == CSNET_OP_MIX || op.kind == CSNET_OP_MIXPROJ) && P.op_tc[i].mt > 0) return Kern::MixTc;
+  if (op.kind == CSNET_OP_MIX && op.n_paths == 1 && op.paths[0].ksize == 0 && op.paths[0].cout0 == 0 && op.paths[0].cout == D.C) {
+    const csnet_path_desc& q = op.paths[0];                    // a pure resample
+    const csnet_tensor_desc& Sq = P.tensors[q.src];
+    const bool avg2 = q.pre_avg == 1 && q.pool == 1, max2 = q.pre_avg == 0 && q.pool == 2;
+    const bool fast = Sq.dtype == D.dtype && D.dtype != CSNET_F32 && D.W % 4 == 0 && op.bias_off < 0 && op.slope_off < 0;
+    if (fast && (avg2 || max2) && q.up == 1 && q.c0 == 0) return Kern::Pool2;
+    if (fast && q.up > 1 && !q.pre_avg && q.pool == 1) return Kern::Upsample;
+    return Kern::Resample;
+  }
+  if (op.kind == CSNET_OP_MIX) return Kern::MixGeneric;
+  if (op.kind == CSNET_OP_GN) return Kern::Gn;
+  if (op.kind == CSNET_OP_ILBLOCK)
+    return make_ils(P, op, &S) && (int64_t)P.max_batch * (D.H / 4) >= (int64_t)P.ils_min_chunks ? Kern::IlStream : Kern::IlBlock;
+  const csnet_tensor_desc& Sd = P.tensors[op.paths[0].src];
+  return op.ext_off[23] != 1 && Sd.dtype == D.dtype && D.dtype != CSNET_F32 && D.W % 4 == 0 ? Kern::DwFast : Kern::DwGeneric;
 }
 
 template <typename T>
@@ -851,40 +864,30 @@ int csnet_plan_create(csnet_plan** out, const csnet_tensor_desc* tensors, int32_
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) == cudaSuccess && prop.multiProcessorCount > 0) P->num_sms = prop.multiProcessorCount;
   }
-  P->op_msd.assign(P->ops.size(), 0);
-  for (size_t i = 0; i < P->ops.size(); ++i) P->op_msd[i] = is_msd(*P, P->ops[i]) ? 1 : 0;
-  if (const char* e6 = getenv("CSNET_GRAPH_MAX_N")) P->graph_max_n = atoi(e6);
-  if (const char* e4 = getenv("CSNET_MS")) P->ms_enabled = e4[0] != '0';
-  P->op_ms.assign(P->ops.size(), 0);
-  bool any_ms = false;
+  // the kernel switches, read when the plan is created: CSNET_MS=0 keeps 1x1 MIX ops off mix_stream, CSNET_ILS=0 keeps
+  // ILBLOCK ops off il_stream, CSNET_ILS_NS forces its column strips and CSNET_ILS_MIN_CHUNKS its batch threshold
+  if (const char* s = getenv("CSNET_MS")) P->ms_enabled = s[0] != '0';
+  if (const char* s = getenv("CSNET_ILS")) P->ils_enabled = s[0] != '0';
+  if (const char* s = getenv("CSNET_ILS_NS")) P->ils_force_ns = atoi(s);
+  P->ils_min_chunks = 4 * P->num_sms;
+  if (const char* s = getenv("CSNET_ILS_MIN_CHUNKS")) P->ils_min_chunks = atoi(s);
+  P->op_kern.resize(P->ops.size());
+  bool any_ms = false, any_ils = false;
   for (size_t i = 0; i < P->ops.size(); ++i) {
-    csnet::MsArgs M;
-    if (make_ms(*P, P->ops[i], 1, nullptr, &M, nullptr)) { P->op_ms[i] = 1; any_ms = true; }
+    P->op_kern[i] = choose_kernel(*P, i);
+    any_ms |= P->op_kern[i] == Kern::MixStream;
+    any_ils |= P->op_kern[i] == Kern::IlStream;
   }
   if (any_ms) {
     e = cudaFuncSetAttribute(csnet::mix_stream_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return cleanup(CSNET_E_CUDA, std::string("cudaFuncSetAttribute(mix_stream): ") + cudaGetErrorString(e));
   }
-  P->op_ils.assign(P->ops.size(), 0);
-  P->ils_min_chunks = 4 * P->num_sms;
-  if (const char* e1 = getenv("CSNET_ILS")) P->ils_enabled = e1[0] != '0';
-  if (const char* e3 = getenv("CSNET_ILS_NS")) P->ils_force_ns = atoi(e3);
-  if (const char* e2 = getenv("CSNET_ILS_MIN_CHUNKS")) P->ils_min_chunks = atoi(e2);
-  int ils_smem_max = 0;
-  for (size_t i = 0; i < P->ops.size(); ++i) {
-    csnet::IlsArgs S;
-    if (!make_ils(*P, P->ops[i], &S)) continue;
-    P->op_ils[i] = 1;
-    ils_smem_max = S.smem_bytes > ils_smem_max ? S.smem_bytes : ils_smem_max;
-  }
-  if (ils_smem_max > 0) {
+  if (any_ils) {
     // always the architectural maximum: plans created later must not lower the limit an earlier plan relies on
     e = cudaFuncSetAttribute(csnet::il_stream_kernel<__half, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::il_stream_kernel<__half, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::il_stream_kernel<__half, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     // two CTAs of <= 113 KB share an SM only with the full shared-memory carve-out
     if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::il_stream_kernel<__half, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::il_stream_kernel<__half, true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     if (e != cudaSuccess) return cleanup(CSNET_E_CUDA, std::string("cudaFuncSetAttribute(il_stream): ") + cudaGetErrorString(e));
   }
   if (P->il_smem_max > 0) {
@@ -947,153 +950,143 @@ static int check_run_args(csnet_plan* P, int32_t N, const void* const* ext_ptrs,
 static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_ptrs, cudaStream_t stream) {
   const csnet_op_desc& op = P->ops[i];
   const csnet_tensor_desc& D = P->tensors[op.dst];
-  if (P->op_msd[i]) {
-    // MSBlock: one launch per dilated path on the FP32 pipe (ms_direct.cuh)
-    for (int p = 0; p < op.n_paths; ++p) {
-      const csnet_path_desc& q = op.paths[p];
-      csnet::MsdArgs A{};
-      A.src = reinterpret_cast<const uint16_t*>(P->tensor_ptr(q.src, N, ext_ptrs));
-      A.dst = reinterpret_cast<uint16_t*>(P->tensor_ptr(op.dst, N, ext_ptrs));
-      A.w = P->blob + q.w_off;
-      A.bias = op.bias_off >= 0 ? P->blob + op.bias_off : nullptr;
-      A.slope = op.slope_off >= 0 ? P->blob + op.slope_off : nullptr;
-      A.N = N; A.Cin = q.cin; A.H = D.H; A.W = D.W; A.Ctot = D.C; A.cout0 = q.cout0; A.cout = q.cout;
-      csnet::msd_launch<__half>(q.dil, A, stream);
+  switch (P->op_kern[i]) {
+    case Kern::Msd:
+      // MSBlock: one launch per dilated path on the FP32 pipe (ms_direct.cuh)
+      for (int p = 0; p < op.n_paths; ++p) {
+        const csnet_path_desc& q = op.paths[p];
+        csnet::MsdArgs A{};
+        A.src = reinterpret_cast<const uint16_t*>(P->tensor_ptr(q.src, N, ext_ptrs));
+        A.dst = reinterpret_cast<uint16_t*>(P->tensor_ptr(op.dst, N, ext_ptrs));
+        A.w = P->blob + q.w_off;
+        A.bias = op.bias_off >= 0 ? P->blob + op.bias_off : nullptr;
+        A.slope = op.slope_off >= 0 ? P->blob + op.slope_off : nullptr;
+        A.N = N; A.Cin = q.cin; A.H = D.H; A.W = D.W; A.Ctot = D.C; A.cout0 = q.cout0; A.cout = q.cout;
+        csnet::msd_launch<__half>(q.dil, A, stream);
+      }
+      break;
+    case Kern::MixStream: {
+      // streaming 1x1 MIX kernel (mix_stream.cuh): TMA operand tiles -> wgmma -> epilogue (resample-adds, PReLU, projection)
+      csnet::MsArgs A;
+      CUtensorMap maps[csnet::kMsMaxIn];
+      memset(maps, 0, sizeof maps);
+      if (!make_ms(*P, op, N, ext_ptrs, &A, maps)) return fail(CSNET_E_UNSUPPORTED, "MIX op no longer qualifies for the streaming kernel");
+      for (int k = A.n_in; k < csnet::kMsMaxIn; ++k) maps[k] = maps[0];
+      int grid = A.total_chunks / 2;
+      grid = grid < 1 ? 1 : (grid > P->num_sms ? P->num_sms : grid);
+      csnet::mix_stream_kernel<__half><<<grid, csnet::kMsThreads, A.smem_bytes, stream>>>(A, maps[0], maps[1], maps[2]);
+      break;
     }
-  } else if (P->op_ms[i] && (int64_t)P->max_batch * (D.H / csnet::kMsRows) >= (int64_t)2 * P->num_sms) {
-    // streaming 1x1 MIX kernel (mix_stream.cuh): TMA operand tiles -> wgmma -> epilogue (resample-adds, PReLU, projection)
-    csnet::MsArgs A;
-    CUtensorMap maps[csnet::kMsMaxIn];
-    memset(maps, 0, sizeof maps);
-    if (!make_ms(*P, op, N, ext_ptrs, &A, maps)) return fail(CSNET_E_UNSUPPORTED, "MIX op no longer qualifies for the streaming kernel");
-    for (int k = A.n_in; k < csnet::kMsMaxIn; ++k) maps[k] = maps[0];
-    int grid = A.total_chunks / 2;
-    grid = grid < 1 ? 1 : (grid > P->num_sms ? P->num_sms : grid);
-    csnet::mix_stream_kernel<__half><<<grid, csnet::kMsThreads, A.smem_bytes, stream>>>(A, maps[0], maps[1], maps[2]);
-  } else if ((op.kind == CSNET_OP_MIX || op.kind == CSNET_OP_MIXPROJ) && P->op_tc[i].mt > 0) {
-    csnet::MixArgs A = make_mix(*P, op, N, ext_ptrs);
-    const TcChoice& tc = P->op_tc[i];
-    const int Cm = A.C;
-    csnet::TcGeom G{};
-    G.tiles_x = (D.W + csnet::kTcTW - 1) / csnet::kTcTW; G.xs_halves = tc.xs_halves; G.kc = tc.kc; G.rows = tc.rows;
-    const int th = csnet::kTcTH * tc.rows;
-    G.m16_total = (Cm + tc.mt * 16 - 1) / (tc.mt * 16) * (tc.mt * 16);
-    for (int p = 0; p < op.n_paths; ++p) G.w16[p] = P->op_w16[i][p];
-    dim3 grid(G.tiles_x * ((D.H + th - 1) / th), (Cm + tc.mt * 16 - 1) / (tc.mt * 16), N);
-    launch_mix_tc(tc, grid, P->op_smem[i], stream, A, G);
-  } else if (op.kind == CSNET_OP_MIX && op.n_paths == 1 && op.paths[0].ksize == 0 && op.paths[0].cout0 == 0 &&
-             op.paths[0].cout == D.C) {
-    csnet::MixArgs A = make_mix(*P, op, N, ext_ptrs);         // a pure resample
-    const csnet_path_desc& q = op.paths[0];
-    const csnet_tensor_desc& S = P->tensors[q.src];
-    const bool avg2 = q.pre_avg == 1 && q.pool == 1, max2 = q.pre_avg == 0 && q.pool == 2;
-    if ((avg2 || max2) && q.up == 1 && q.c0 == 0 && S.dtype == D.dtype && D.dtype != CSNET_F32 && D.W % 4 == 0 &&
-        op.bias_off < 0 && op.slope_off < 0) {
+    case Kern::MixTc: {
+      csnet::MixArgs A = make_mix(*P, op, N, ext_ptrs);
+      const TcChoice& tc = P->op_tc[i];
+      const int Cm = A.C;
+      csnet::TcGeom G{};
+      G.tiles_x = (D.W + csnet::kTcTW - 1) / csnet::kTcTW; G.xs_halves = tc.xs_halves; G.kc = tc.kc; G.rows = tc.rows;
+      const int th = csnet::kTcTH * tc.rows;
+      G.m16_total = (Cm + tc.mt * 16 - 1) / (tc.mt * 16) * (tc.mt * 16);
+      for (int p = 0; p < op.n_paths; ++p) G.w16[p] = P->op_w16[i][p];
+      dim3 grid(G.tiles_x * ((D.H + th - 1) / th), (Cm + tc.mt * 16 - 1) / (tc.mt * 16), N);
+      launch_mix_tc(tc, grid, P->op_smem[i], stream, A, G);
+      break;
+    }
+    case Kern::Pool2: {
+      csnet::MixArgs A = make_mix(*P, op, N, ext_ptrs);
+      const bool max2 = op.paths[0].pool == 2;
       const dim3 grid((D.H * (D.W / 4) + 255) / 256, D.C, N);    // avg_pool2d(2, 2) / max_pool2d(2, 2) of a 16-bit tensor
       if (D.dtype == CSNET_F16) csnet::pool2_fast_kernel<__half><<<grid, 256, 0, stream>>>(A, max2);
       else csnet::pool2_fast_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(A, max2);
-    } else if (q.up > 1 && !q.pre_avg && q.pool == 1 && S.dtype == D.dtype && D.dtype != CSNET_F32 && D.W % 4 == 0 &&
-               op.bias_off < 0 && op.slope_off < 0) {
+      break;
+    }
+    case Kern::Upsample: {
+      csnet::MixArgs A = make_mix(*P, op, N, ext_ptrs);
       const dim3 grid((D.H * (D.W / 4) + 255) / 256, D.C, N);    // bilinear up-sampling, 16-bit to 16-bit
       if (D.dtype == CSNET_F16) csnet::upsample_fast_kernel<__half><<<grid, 256, 0, stream>>>(A);
       else csnet::upsample_fast_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(A);
-    } else {
-      csnet::resample_fast_kernel<<<dim3((D.H * D.W + 255) / 256, D.C, N), 256, 0, stream>>>(A);
+      break;
     }
-  } else if (op.kind == CSNET_OP_MIX) {
-    csnet::MixArgs A = make_mix(*P, op, N, ext_ptrs);
-    dim3 grid((D.H * D.W + kThreads - 1) / kThreads, (D.C + csnet::kMixCT - 1) / csnet::kMixCT, N);
-    mix_generic_kernel<<<grid, kThreads, 0, stream>>>(A);
-  } else if (op.kind == CSNET_OP_GN) {
-    const csnet_tensor_desc& S = P->tensors[op.paths[0].src];
-    csnet::GnArgs A{};
-    A.src = P->tensor_ptr(op.paths[0].src, N, ext_ptrs);
-    A.dst = P->tensor_ptr(op.dst, N, ext_ptrs);
-    A.gamma = P->blob + op.ext_off[0];
-    A.beta = P->blob + op.ext_off[1];
-    A.slope = op.slope_off >= 0 ? P->blob + op.slope_off : nullptr;
-    A.stats = P->gn_stats;
-    A.src_dtype = S.dtype; A.dst_dtype = D.dtype; A.C = D.C; A.HW = D.H * D.W; A.groups = op.paths[0].up;
-    gn_stats_kernel<<<dim3(A.groups, N), kThreads, 0, stream>>>(A);
-    const int bx = (A.HW + kThreads * 4 - 1) / (kThreads * 4);
-    gn_apply_kernel<<<dim3(bx < 1 ? 1 : bx, D.C, N), kThreads, 0, stream>>>(A);
-  } else if (op.kind == CSNET_OP_ILBLOCK && P->op_ils[i] && (int64_t)P->max_batch * (D.H / 4) >= (int64_t)P->ils_min_chunks) {
-    // (the choice depends on the plan's max_batch, not on N: every sub-batch of a plan runs the same kernels, bit for bit)
-    // streaming kernel (il_stream.cuh): TMA operand tiles, wgmma GEMM, register-resident depthwise tail
-    csnet::IlsArgs A;
-    if (!make_ils(*P, op, &A)) return fail(CSNET_E_UNSUPPORTED, "ILBLOCK op no longer qualifies for the streaming kernel");
-    auto f = [&](int e) { return op.ext_off[e] >= 0 ? P->blob + op.ext_off[e] : nullptr; };
-    A.yh = P->tensor_ptr(op.dst, N, ext_ptrs);
-    A.yl = op.dst2 >= 0 ? P->tensor_ptr(op.dst2, N, ext_ptrs) : nullptr;
-    A.wh = reinterpret_cast<const uint32_t*>(f(0));
-    A.wl = reinterpret_cast<const uint32_t*>(f(1));
-    A.dw1h = {f(6), f(7), f(8)};   A.dw1l = {f(9), f(10), f(11)};
-    A.dw2h = {f(12), f(13), f(14)}; A.dw2l = {f(15), f(16), f(17)};
-    A.N = N;
-    A.total_chunks = N * A.ns * A.cpi;
-    CUtensorMap tmH, tmL;
-    const bool stem = A.Ci > 0;
-    if (stem) {
-      if (!encode_image_map(&tmL, P->tensor_ptr(op.paths[0].src, N, ext_ptrs), N, A.Ci, A.H, A.W, A.BW, 4)) 
-        return fail(CSNET_E_CUDA, "cuTensorMapEncodeTiled failed (streaming ILBlock, image)");
-      tmH = tmL;
-    } else if (!encode_group_map(&tmH, P->tensor_ptr(op.paths[0].src, N, ext_ptrs), N, A.Chi, A.H, A.W, A.SH, A.GR, 4) ||
-               !encode_group_map(&tmL, P->tensor_ptr(op.paths[1].src, N, ext_ptrs), N, A.Cli, A.H / 2, A.W / 2, A.SL, A.GLR, 2))
-      return fail(CSNET_E_CUDA, "cuTensorMapEncodeTiled failed (streaming ILBlock)");
-    int grid = A.total_chunks / 4;
-    grid = grid < 1 ? 1 : (grid > P->num_sms ? P->num_sms : grid);     // persistent: one CTA per SM
-    static const bool dbg = [] { const char* e = getenv("CSNET_ILS_DBG"); return e && e[0] == '1'; }();
-    static unsigned long long* dbg_buf = nullptr;
-    if (dbg && !dbg_buf) cudaMalloc(&dbg_buf, 1024 * 8 * sizeof(unsigned long long));
-    A.dbg = dbg ? dbg_buf : nullptr;
-    if (stem) csnet::il_stream_kernel<__half, false, true><<<grid, A.dw_warps * 32, A.smem_bytes, stream>>>(A, tmH, tmL);
-    else if (dbg) csnet::il_stream_kernel<__half, true><<<grid, A.dw_warps * 32, A.smem_bytes, stream>>>(A, tmH, tmL);
-    else csnet::il_stream_kernel<__half, false><<<grid, A.dw_warps * 32, A.smem_bytes, stream>>>(A, tmH, tmL);
-    if (dbg && !stem) {        // debugging aid: mean cycles per phase over the CTAs (synchronises)
-      std::vector<unsigned long long> h((size_t)grid * 8);
-      cudaStreamSynchronize(stream);
-      cudaMemcpy(h.data(), dbg_buf, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-      double m[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      for (int b = 0; b < grid; ++b) for (int k = 0; k < 8; ++k) m[k] += (double)h[(size_t)b * 8 + k] / grid;
-      int occ = -1;
-      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, csnet::il_stream_kernel<__half, true>, A.dw_warps * 32, A.smem_bytes);
-      fprintf(stderr, "[ils ns %d grid %d threads %d smem %d occupancy %d] ", A.ns, grid, A.dw_warps * 32, A.smem_bytes, occ);
-      fprintf(stderr, "[ils %dx%d C %d+%d->%d+%d] cycles/CTA: load-wait %.0f resample %.0f syncA %.0f issue %.0f epilogue %.0f syncB %.0f dw %.0f tail %.0f\n",
-              A.H, A.W, A.Chi, A.Cli, A.Cho, A.Clo, m[0], m[1], m[2], m[3], m[4], m[5], m[6], m[7]);
+    case Kern::Resample:
+      csnet::resample_fast_kernel<<<dim3((D.H * D.W + 255) / 256, D.C, N), 256, 0, stream>>>(make_mix(*P, op, N, ext_ptrs));
+      break;
+    case Kern::MixGeneric: {
+      dim3 grid((D.H * D.W + kThreads - 1) / kThreads, (D.C + csnet::kMixCT - 1) / csnet::kMixCT, N);
+      mix_generic_kernel<<<grid, kThreads, 0, stream>>>(make_mix(*P, op, N, ext_ptrs));
+      break;
     }
-  } else if (op.kind == CSNET_OP_ILBLOCK) {
-    csnet::IlArgs A;
-    if (!make_il(*P, op, N, ext_ptrs, &A)) return fail(CSNET_E_UNSUPPORTED, "ILBLOCK op does not fit shared memory");
-    const int tiles_y = (A.H + A.TH - 1) / A.TH;
-    dim3 grid(A.tiles_x * tiles_y, 1, N);
-    CUtensorMap tmH, tmL;
-    memset(&tmH, 0, sizeof tmH);
-    memset(&tmL, 0, sizeof tmL);
-    if (A.tma_h && !encode_plane_map(&tmH, A.xh, N, A.Chi, A.H, A.W, A.TW + 8, (A.TH + 8) | 1, A.Chi))
-      return fail(CSNET_E_CUDA, "cuTensorMapEncodeTiled failed (hi input)");
-    if (A.tma_l && !encode_plane_map(&tmL, A.xl, N, A.Cli, A.H / 2, A.W / 2, A.TW / 2 + 8, (A.TH / 2 + 4) | 1, A.Cli))
-      return fail(CSNET_E_CUDA, "cuTensorMapEncodeTiled failed (lo input)");
-    if (D.dtype == CSNET_F16) launch_il_t<__half>(A, grid, P->op_smem[i], stream, tmH, tmL);
-    else launch_il_t<__nv_bfloat16>(A, grid, P->op_smem[i], stream, tmH, tmL);
-  } else {
-    const csnet_path_desc& q = op.paths[0];
-    const csnet_tensor_desc& S = P->tensors[q.src];
-    csnet::DwArgs A{};
-    A.src = P->tensor_ptr(q.src, N, ext_ptrs);
-    A.dst = P->tensor_ptr(op.dst, N, ext_ptrs);
-    A.w = P->blob + q.w_off;
-    A.bias = op.bias_off >= 0 ? P->blob + op.bias_off : nullptr;
-    A.slope = op.slope_off >= 0 ? P->blob + op.slope_off : nullptr;
-    A.src_dtype = S.dtype; A.dst_dtype = D.dtype; A.C = D.C; A.H = D.H; A.W = D.W;
-    if (op.ext_off[23] != 1 && S.dtype == D.dtype && D.dtype != CSNET_F32 && D.W % 4 == 0) {
-      const int tasks = (D.W / 4) * ((D.H + csnet::kDwfRun - 1) / csnet::kDwfRun);
-      dim3 grid((tasks + csnet::kDwfThreads - 1) / csnet::kDwfThreads, D.C, N);
-      if (D.dtype == CSNET_F16) csnet::dw_fast_kernel<__half><<<grid, csnet::kDwfThreads, 0, stream>>>(A);
-      else csnet::dw_fast_kernel<__nv_bfloat16><<<grid, csnet::kDwfThreads, 0, stream>>>(A);
-    } else {
-      const int strips = (D.H + csnet::kDwRows - 1) / csnet::kDwRows;
-      dim3 grid((strips * D.W + kThreads - 1) / kThreads, D.C, N);
-      dw_generic_kernel<<<grid, kThreads, 0, stream>>>(A);
+    case Kern::Gn: {
+      const csnet_tensor_desc& S = P->tensors[op.paths[0].src];
+      csnet::GnArgs A{};
+      A.src = P->tensor_ptr(op.paths[0].src, N, ext_ptrs);
+      A.dst = P->tensor_ptr(op.dst, N, ext_ptrs);
+      A.gamma = P->blob + op.ext_off[0];
+      A.beta = P->blob + op.ext_off[1];
+      A.slope = op.slope_off >= 0 ? P->blob + op.slope_off : nullptr;
+      A.stats = P->gn_stats;
+      A.src_dtype = S.dtype; A.dst_dtype = D.dtype; A.C = D.C; A.HW = D.H * D.W; A.groups = op.paths[0].up;
+      gn_stats_kernel<<<dim3(A.groups, N), kThreads, 0, stream>>>(A);
+      const int bx = (A.HW + kThreads * 4 - 1) / (kThreads * 4);
+      gn_apply_kernel<<<dim3(bx < 1 ? 1 : bx, D.C, N), kThreads, 0, stream>>>(A);
+      break;
+    }
+    case Kern::IlStream: {
+      // streaming kernel (il_stream.cuh): TMA operand tiles, wgmma GEMM, register-resident depthwise tail
+      csnet::IlsArgs A;
+      if (!make_ils(*P, op, &A)) return fail(CSNET_E_UNSUPPORTED, "ILBLOCK op no longer qualifies for the streaming kernel");
+      auto f = [&](int e) { return op.ext_off[e] >= 0 ? P->blob + op.ext_off[e] : nullptr; };
+      A.yh = P->tensor_ptr(op.dst, N, ext_ptrs);
+      A.yl = op.dst2 >= 0 ? P->tensor_ptr(op.dst2, N, ext_ptrs) : nullptr;
+      A.wh = reinterpret_cast<const uint32_t*>(f(0));
+      A.wl = reinterpret_cast<const uint32_t*>(f(1));
+      A.dw1h = {f(6), f(7), f(8)};   A.dw1l = {f(9), f(10), f(11)};
+      A.dw2h = {f(12), f(13), f(14)}; A.dw2l = {f(15), f(16), f(17)};
+      A.N = N;
+      A.total_chunks = N * A.ns * A.cpi;
+      CUtensorMap tmH, tmL;
+      const bool stem = A.Ci > 0;
+      if (stem) {
+        if (!encode_image_map(&tmL, P->tensor_ptr(op.paths[0].src, N, ext_ptrs), N, A.Ci, A.H, A.W, A.BW, 4))
+          return fail(CSNET_E_CUDA, "cuTensorMapEncodeTiled failed (streaming ILBlock, image)");
+        tmH = tmL;
+      } else if (!encode_group_map(&tmH, P->tensor_ptr(op.paths[0].src, N, ext_ptrs), N, A.Chi, A.H, A.W, A.SH, A.GR, 4) ||
+                 !encode_group_map(&tmL, P->tensor_ptr(op.paths[1].src, N, ext_ptrs), N, A.Cli, A.H / 2, A.W / 2, A.SL, A.GLR, 2))
+        return fail(CSNET_E_CUDA, "cuTensorMapEncodeTiled failed (streaming ILBlock)");
+      int grid = A.total_chunks / 4;
+      grid = grid < 1 ? 1 : (grid > P->num_sms ? P->num_sms : grid);     // persistent: one CTA per SM
+      if (stem) csnet::il_stream_kernel<__half, true><<<grid, A.dw_warps * 32, A.smem_bytes, stream>>>(A, tmH, tmL);
+      else csnet::il_stream_kernel<__half, false><<<grid, A.dw_warps * 32, A.smem_bytes, stream>>>(A, tmH, tmL);
+      break;
+    }
+    case Kern::IlBlock: {
+      csnet::IlArgs A;
+      if (!make_il(*P, op, N, ext_ptrs, &A)) return fail(CSNET_E_UNSUPPORTED, "ILBLOCK op does not fit shared memory");
+      const int tiles_y = (A.H + A.TH - 1) / A.TH;
+      dim3 grid(A.tiles_x * tiles_y, 1, N);
+      if (D.dtype == CSNET_F16) launch_il_t<__half>(A, grid, P->op_smem[i], stream);
+      else launch_il_t<__nv_bfloat16>(A, grid, P->op_smem[i], stream);
+      break;
+    }
+    case Kern::DwFast:
+    case Kern::DwGeneric: {
+      const csnet_path_desc& q = op.paths[0];
+      const csnet_tensor_desc& S = P->tensors[q.src];
+      csnet::DwArgs A{};
+      A.src = P->tensor_ptr(q.src, N, ext_ptrs);
+      A.dst = P->tensor_ptr(op.dst, N, ext_ptrs);
+      A.w = P->blob + q.w_off;
+      A.bias = op.bias_off >= 0 ? P->blob + op.bias_off : nullptr;
+      A.slope = op.slope_off >= 0 ? P->blob + op.slope_off : nullptr;
+      A.src_dtype = S.dtype; A.dst_dtype = D.dtype; A.C = D.C; A.H = D.H; A.W = D.W;
+      if (P->op_kern[i] == Kern::DwFast) {
+        const int tasks = (D.W / 4) * ((D.H + csnet::kDwfRun - 1) / csnet::kDwfRun);
+        dim3 grid((tasks + csnet::kDwfThreads - 1) / csnet::kDwfThreads, D.C, N);
+        if (D.dtype == CSNET_F16) csnet::dw_fast_kernel<__half><<<grid, csnet::kDwfThreads, 0, stream>>>(A);
+        else csnet::dw_fast_kernel<__nv_bfloat16><<<grid, csnet::kDwfThreads, 0, stream>>>(A);
+      } else {
+        const int strips = (D.H + csnet::kDwRows - 1) / csnet::kDwRows;
+        dim3 grid((strips * D.W + kThreads - 1) / kThreads, D.C, N);
+        dw_generic_kernel<<<grid, kThreads, 0, stream>>>(A);
+      }
+      break;
     }
   }
   CU_CHECK(cudaGetLastError());
@@ -1160,7 +1153,7 @@ int csnet_plan_run(csnet_plan* P, int32_t N, const void* const* ext_ptrs, int32_
   cudaStream_t stream = (cudaStream_t)stream_;
   DeviceGuard guard_(P->device);
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  if (N <= P->graph_max_n && P->n_ext == 2 && cudaStreamIsCapturing(stream, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone)
+  if (N <= kGraphMaxN && P->n_ext == 2 && cudaStreamIsCapturing(stream, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone)
     return run_graph(P, N, ext_ptrs, stream);
   return run_ops(P, N, ext_ptrs, stream);
 }
@@ -1203,31 +1196,22 @@ int csnet_plan_read_tensor(csnet_plan* P, int32_t tensor, int32_t N, void* dst, 
   return CSNET_OK;
 }
 
-// Which kernel launch_op() runs for op i — the same decision chain, by name (bench.py groups per-op times by kernel).
+// Which kernel launch_op() runs for op i, by name (bench.py groups per-op times by kernel).
 const char* csnet_plan_op_kernel(const csnet_plan* P, int32_t i) {
+  static const char* const names[] = {
+      "msd_kernel (ms_direct.cuh, FP32 pipe)", "mix_stream_kernel (TMA + wgmma)", "mix_tc_kernel (mma.sync)",
+      "pool2 / upsample / resample kernels", "pool2 / upsample / resample kernels", "pool2 / upsample / resample kernels",
+      "mix_generic_kernel", "gn kernels", "il_stream_kernel (TMA + wgmma)", "il_block_kernel (mma.sync, tiled)", "dw kernels", "dw kernels"};
+  static_assert(sizeof names / sizeof names[0] == (size_t)Kern::DwGeneric + 1, "one name per Kern");
   if (!P || i < 0 || i >= (int32_t)P->ops.size()) return "";
-  const csnet_op_desc& op = P->ops[i];
-  const csnet_tensor_desc& D = P->tensors[op.dst];
-  if (P->op_msd[i]) return "msd_kernel (ms_direct.cuh, FP32 pipe)";
-  if (P->op_ms[i] && (int64_t)P->max_batch * (D.H / csnet::kMsRows) >= (int64_t)2 * P->num_sms) return "mix_stream_kernel (TMA + wgmma)";
-  if ((op.kind == CSNET_OP_MIX || op.kind == CSNET_OP_MIXPROJ) && P->op_tc[i].mt > 0) return "mix_tc_kernel (mma.sync)";
-  if (op.kind == CSNET_OP_MIX && op.n_paths == 1 && op.paths[0].ksize == 0 && op.paths[0].cout0 == 0 && op.paths[0].cout == D.C)
-    return "pool2 / upsample / resample kernels";
-  if (op.kind == CSNET_OP_MIX) return "mix_generic_kernel";
-  if (op.kind == CSNET_OP_GN) return "gn kernels";
-  if (op.kind == CSNET_OP_ILBLOCK && P->op_ils[i] && (int64_t)P->max_batch * (D.H / 4) >= (int64_t)P->ils_min_chunks)
-    return "il_stream_kernel (TMA + wgmma)";
-  if (op.kind == CSNET_OP_ILBLOCK) return "il_block_kernel (mma.sync, tiled)";
-  return "dw kernels";
+  return names[(int)P->op_kern[i]];
 }
 
 int32_t csnet_plan_launches(const csnet_plan* P) {
   if (!P) return 0;
   int32_t n = 0;
-  for (size_t i = 0; i < P->ops.size(); ++i) {
-    const auto& op = P->ops[i];
-    n += op.kind == CSNET_OP_GN ? 2 : (i < P->op_msd.size() && P->op_msd[i] ? op.n_paths : 1);
-  }
+  for (size_t i = 0; i < P->ops.size(); ++i)
+    n += P->op_kern[i] == Kern::Gn ? 2 : (P->op_kern[i] == Kern::Msd ? P->ops[i].n_paths : 1);
   return n;
 }
 
@@ -1285,59 +1269,16 @@ static int run_host_impl(csnet_plan* P, int32_t N, const void* x_host, void* y_h
   // The batch is cut into chunks that flow through a three-stage pipeline: H2D copy (own stream) -> program
   // (caller's stream) -> D2H copy (own stream), with ping-pong device staging, so the PCIe copies of chunk i+1 / i-1
   // overlap the kernels of chunk i.  Pinned host memory is needed for the copies to be truly asynchronous.
-  // Schedule: a small first and last chunk (N/8 images) keep the exposed copies short — the first H2D and the last D2H are
-  // the only ones nothing overlaps — and one large middle chunk keeps the kernels at large-batch efficiency (measured at
-  // bs 256: 4 equal chunks 25.2 ms, 2 equal 24.5 ms).  CSNET_HOST_CHUNKS=k forces k equal chunks.
-  static const int n_equal = [] { const char* e = getenv("CSNET_HOST_CHUNKS"); const int v = e ? atoi(e) : 0; return v < 0 ? 0 : (v > 16 ? 16 : v); }();
-  static int sched[2][16], sched_n[2] = {0, 0};
-  static const bool sched_parsed = [] {
-    const char* names[2] = {"CSNET_HOST_SCHED", "CSNET_HOST_SCHED_U8"};
-    for (int k = 0; k < 2; ++k) {
-      const char* e = getenv(names[k]);
-      int tot = 0;
-      while (e && *e && sched_n[k] < 16) {
-        const int v = atoi(e);
-        if (v <= 0) { sched_n[k] = 0; break; }
-        sched[k][sched_n[k]++] = v; tot += v;
-        e = strchr(e, ',');
-        if (e) ++e;
-      }
-      if (tot != 256) sched_n[k] = 0;
-    }
-    return true; }();
-  (void)sched_parsed;
-  int sizes[16], n_sizes = 0;
-  if (N < 64) {
-    sizes[n_sizes++] = N;
-  } else if (sched_n[u8 ? 1 : 0] > 0) {
-    // explicit schedule in 256ths of the batch (CSNET_HOST_SCHED / CSNET_HOST_SCHED_U8 = "16,32,64,112,32"); the rounding remainder
-    // goes to the largest chunk.  Measured (scripts/host_split.py, bs 256): every ramp with 4-6 chunks is SLOWER than the default
-    // 32 / 192 / 32 (17.3-20.0 ms vs 16.5 ms) — each extra chunk pays the 81 launches again at a small batch.
-    const int* v = sched[u8 ? 1 : 0];
-    int tot = 0, big = 0;
-    for (int i = 0; i < sched_n[u8 ? 1 : 0]; ++i) { sizes[n_sizes] = N * v[i] / 256; tot += sizes[n_sizes]; if (sizes[n_sizes] > sizes[big]) big = n_sizes; ++n_sizes; }
-    sizes[big] += N - tot;
-    int k = 0;
-    for (int i = 0; i < n_sizes; ++i) if (sizes[i] > 0) sizes[k++] = sizes[i];
-    n_sizes = k;
-  } else if (n_equal > 0) {
-    const int c = (N + n_equal - 1) / n_equal;
-    for (int n0 = 0; n0 < N; n0 += c) sizes[n_sizes++] = (N - n0) < c ? (N - n0) : c;
-  } else {
-    // first / last chunk in 256ths of the batch (CSNET_HOST_SPLIT="first,last", 0 = no such chunk); default 32 / 32
-    // (uint8 form: the copies are 4x smaller, so one chunk at full-batch kernel efficiency wins; CSNET_HOST_SPLIT_U8)
-    static int f256 = 32, l256 = 32, f256u = 0, l256u = 0;    // measured (scripts/host_split.py): u8 one chunk 14.7 ms, 32/32 16.1 ms
-    static const bool parsed = [] {
-      const char* e = getenv("CSNET_HOST_SPLIT"); if (e) sscanf(e, "%d,%d", &f256, &l256);
-      e = getenv("CSNET_HOST_SPLIT_U8"); if (e) sscanf(e, "%d,%d", &f256u, &l256u);
-      return true; }();
-    (void)parsed;
-    const int first = N * (u8 ? f256u : f256) / 256, last = N * (u8 ? l256u : l256) / 256;
-    if (first > 0 && first < N) sizes[n_sizes++] = first;
-    const int mid = N - (first > 0 && first < N ? first : 0) - (last > 0 && last < N - first ? last : 0);
-    sizes[n_sizes++] = mid;
-    if (last > 0 && last < N - first) sizes[n_sizes++] = last;
-  }
+  // Schedule: batches under 64 images run as one chunk.  Larger fp32 batches run a small first and last chunk (N/8 images)
+  // that keep the exposed copies short — the first H2D and the last D2H are the only ones nothing overlaps — and one large
+  // middle chunk that keeps the kernels at large-batch efficiency.  The uint8 form's copies are 4x smaller: one chunk.
+  // Measured at bs 256: fp32 32 / 192 / 32 16.5 ms (4 equal chunks 25.2 ms, 2 equal 24.5 ms, ramps of 4-6 chunks 17.3-20.0 ms);
+  // uint8 one chunk 14.7 ms (32 / 192 / 32 16.1 ms).
+  const int edge = N < 64 || u8 ? 0 : N * 32 / 256;
+  int sizes[3], n_sizes = 0;
+  if (edge > 0) sizes[n_sizes++] = edge;
+  sizes[n_sizes++] = N - 2 * edge;
+  if (edge > 0) sizes[n_sizes++] = edge;
   int chunk = 0;
   for (int i = 0; i < n_sizes; ++i) chunk = sizes[i] > chunk ? sizes[i] : chunk;
   const size_t xin = (size_t)in->C * in->H * in->W * sizeof(float), yout = (size_t)lo->C * lo->H * lo->W * sizeof(float);

@@ -106,40 +106,6 @@ __global__ void __launch_bounds__(kT) bn_stats_kernel(const float* __restrict__ 
   }
 }
 
-// stats: per channel mean and biased variance.  Each part is reduced two-pass (its own mean first), parts are merged with
-// Chan's formula: M2 = sum M2_p + sum m_p (mean_p - mean)^2.
-__global__ void __launch_bounds__(kT) bn_stats2_kernel(const float* __restrict__ z, int N, int C, int HW, int S, float* mean,
-                                                      float* var, float* ws, unsigned* cnt) {
-  const int c = blockIdx.x, part = blockIdx.y, parts = gridDim.y, n = part / S, sg = part - n * S;
-  const int seg = (HW + S - 1) / S, i0 = sg * seg, i1 = (i0 + seg) < HW ? (i0 + seg) : HW;
-  const float* p = z + ((size_t)n * C + c) * HW;
-  float s = 0.f, d0 = 0.f, d1 = 0.f;
-  for (int i = i0 + threadIdx.x; i < i1; i += kT) s += p[i];
-  block_sum3(s, d0, d1);
-  __shared__ float mu_s;
-  const float m = (float)(i1 > i0 ? i1 - i0 : 0);
-  if (threadIdx.x == 0) mu_s = m > 0.f ? s / m : 0.f;
-  __syncthreads();
-  const float mu = mu_s;
-  float q = 0.f;
-  for (int i = i0 + threadIdx.x; i < i1; i += kT) { const float d = p[i] - mu; q += d * d; }
-  block_sum3(q, d0, d1);
-  float* w = ws + ((size_t)c * parts + part) * 3;
-  if (threadIdx.x == 0) { w[0] = mu; w[1] = q; w[2] = m; }
-  if (!last_block_of(cnt + c, parts)) return;
-  if (threadIdx.x == 0) {
-    __threadfence();
-    const volatile float* v = ws + (size_t)c * parts * 3;
-    float tot = 0.f, acc = 0.f;
-    for (int k = 0; k < parts; ++k) { tot += v[3 * k + 2]; acc += v[3 * k + 2] * v[3 * k]; }
-    const float mean_c = acc / tot;
-    float m2 = 0.f;
-    for (int k = 0; k < parts; ++k) { const float d = v[3 * k] - mean_c; m2 += v[3 * k + 1] + v[3 * k + 2] * d * d; }
-    mean[c] = mean_c; var[c] = m2 / tot;
-    cnt[c] = 0u;                                            // ready for the next call on this stream
-  }
-}
-
 // y = prelu(gamma * (z - mean) * rsqrt(var + eps) + beta);  gap[n*C+c] = mean over HW of y (optional)
 __global__ void __launch_bounds__(kT) bn_prelu_fwd_kernel(const float* __restrict__ z, float* __restrict__ y, int C, int HW,
                                                           const float* mean, const float* var, const float* gamma,
@@ -210,47 +176,6 @@ __global__ void __launch_bounds__(kT) bn_prelu_bwd_apply_kernel(const float* __r
     const float du = u > 0.f ? d : a * d;
     dz[off + i] = g * r * (du - m1 - xh * m2);
   }
-}
-
-// ---- depthwise 3x3 (Conv2dX100: effective weight = scale * w) ---------------------------------------------
-__global__ void __launch_bounds__(kT) dw_fwd_kernel(const float* __restrict__ x, const float* __restrict__ w, float* __restrict__ y,
-                                                    int C, int H, int W, float scale, int flip) {
-  const int c = blockIdx.y, n = blockIdx.z;
-  const int pix = blockIdx.x * kT + threadIdx.x;
-  if (pix >= H * W) return;
-  const int oy = pix / W, ox = pix % W;
-  const float* p = x + ((size_t)n * C + c) * H * W;
-  float acc = 0.f;
-#pragma unroll
-  for (int ky = 0; ky < 3; ++ky) {
-    const int yy = oy + ky - 1;
-    if (yy < 0 || yy >= H) continue;
-#pragma unroll
-    for (int kx = 0; kx < 3; ++kx) {
-      const int xx = ox + kx - 1;
-      if (xx < 0 || xx >= W) continue;
-      const int t = flip ? (2 - ky) * 3 + (2 - kx) : ky * 3 + kx;   // flip: transposed conv = data gradient
-      acc += p[(size_t)yy * W + xx] * w[c * 9 + t];
-    }
-  }
-  y[((size_t)n * C + c) * H * W + pix] = acc * scale;
-}
-
-// dw[c][tap] = scale * sum_{n,y,x} dy[y,x] * x[y+ky-1, x+kx-1]
-__global__ void __launch_bounds__(kT) dw_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dy, float* dw, int N,
-                                                      int C, int H, int W, float scale) {
-  const int c = blockIdx.x, tap = blockIdx.y, ky = tap / 3, kx = tap % 3;
-  float s = 0.f, d0 = 0.f, d1 = 0.f;
-  for (int n = 0; n < N; ++n) {
-    const float* p = x + ((size_t)n * C + c) * H * W;
-    const float* q = dy + ((size_t)n * C + c) * H * W;
-    for (int i = threadIdx.x; i < H * W; i += kT) {
-      const int oy = i / W, ox = i % W, yy = oy + ky - 1, xx = ox + kx - 1;
-      if (yy >= 0 && yy < H && xx >= 0 && xx < W) s += q[i] * p[(size_t)yy * W + xx];
-    }
-  }
-  block_sum3(s, d0, d1);
-  if (threadIdx.x == 0) dw[c * 9 + tap] = s * scale;
 }
 
 // ---- MIX forward (raw: no bias / slope) -----------------------------------------------------------------------
@@ -540,11 +465,6 @@ constexpr size_t kFastSmem = 92 * 1024;                   // operand tiles; + kF
 constexpr size_t kFastWsm = 16 * 1024;
 constexpr int kFastSmemMax = (int)(kFastSmem + kFastWsm);
 
-static bool fast_enabled() {
-  static const bool on = [] { const char* e = getenv("CSNET_TRAIN_FAST"); return !(e && e[0] == '0'); }();
-  return on;
-}
-
 static int current_device() {
   int dev = 0;
   cudaGetDevice(&dev);
@@ -615,9 +535,8 @@ static int launch_conv1x1(const tf::ConvArgs& F, cudaStream_t st) {
   const size_t tasks = (size_t)A.N * A.H * A.quads;
   const unsigned blocks = (unsigned)((tasks + tf::kT - 1) / tf::kT);
   // <= 24 output channels: the narrow form (8 channels per pass, three CTAs per SM) hides the load latency a little better
-  // (18 -> 18 @224^2 0.494 -> 0.472 ms, 13 -> 18 0.415 -> 0.357 ms; 34 -> 31 @112^2 is 8 % slower with it).  CSNET_C1_NARROW=0 / 1 forces.
-  static const int narrow_env = [] { const char* e = getenv("CSNET_C1_NARROW"); return e ? (e[0] == '1' ? 1 : 0) : -1; }();
-  const bool narrow = narrow_env >= 0 ? narrow_env == 1 : A.C <= 24;
+  // (18 -> 18 @224^2 0.494 -> 0.472 ms, 13 -> 18 0.415 -> 0.357 ms; 34 -> 31 @112^2 is 8 % slower with it).
+  const bool narrow = A.C <= 24;
   static bool attr_n_dev[kMaxDevices] = {false};
   bool& attr_n = attr_n_dev[current_device()];
   if (narrow && !attr_n) { cudaFuncSetAttribute(tf::conv1x1_narrow_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 72 * 1024); attr_n = true; }
@@ -677,9 +596,7 @@ static int reduce_segments(int N, int C, int HW) {
 int csnet_train_bn_stats(const float* z, int32_t N, int32_t C, int32_t HW, float* mean, float* var, void* stream) {
   const int S = reduce_segments(N, C, HW);
   if (int rc = reduce_workspace(C, N * S, (cudaStream_t)stream)) return rc;
-  static const bool two_pass = [] { const char* e = getenv("CSNET_BN_TWO_PASS"); return e && e[0] == '1'; }();
-  if (two_pass) bn_stats2_kernel<<<dim3(C, N * S), kT, 0, (cudaStream_t)stream>>>(z, N, C, HW, S, mean, var, g_red_ws, g_red_cnt);
-  else bn_stats_kernel<<<dim3(C, N * S), kT, 0, (cudaStream_t)stream>>>(z, N, C, HW, S, mean, var, g_red_ws, g_red_cnt);
+  bn_stats_kernel<<<dim3(C, N * S), kT, 0, (cudaStream_t)stream>>>(z, N, C, HW, S, mean, var, g_red_ws, g_red_cnt);
   TR_CHECK(cudaGetLastError());
   return CSNET_OK;
 }
@@ -706,32 +623,24 @@ int csnet_train_bn_prelu_bwd(const float* z, const float* dy, float* dz, int32_t
 
 int csnet_train_dw_conv(const float* x, const float* w, float* y, int32_t N, int32_t C, int32_t H, int32_t W, float scale,
                         int32_t transposed, void* stream) {
-  if (fast_enabled()) {
-    const int quads = (W + 3) / 4, rows = H < 8 ? H : 8, bands = (H + rows - 1) / rows;
-    const size_t tasks = (size_t)N * C * bands * quads;
-    tf::dw3_kernel<<<(unsigned)((tasks + tf::kT - 1) / tf::kT), tf::kT, 0, (cudaStream_t)stream>>>(x, w, y, N, C, H, W, scale, transposed, quads, rows);
-  } else {
-    dw_fwd_kernel<<<dim3((H * W + kT - 1) / kT, C, N), kT, 0, (cudaStream_t)stream>>>(x, w, y, C, H, W, scale, transposed);
-  }
+  const int quads = (W + 3) / 4, rows = H < 8 ? H : 8, bands = (H + rows - 1) / rows;
+  const size_t tasks = (size_t)N * C * bands * quads;
+  tf::dw3_kernel<<<(unsigned)((tasks + tf::kT - 1) / tf::kT), tf::kT, 0, (cudaStream_t)stream>>>(x, w, y, N, C, H, W, scale, transposed, quads, rows);
   TR_CHECK(cudaGetLastError());
   return CSNET_OK;
 }
 
 int csnet_train_dw_wgrad(const float* x, const float* dy, float* dw, int32_t N, int32_t C, int32_t H, int32_t W, float scale, void* stream) {
-  if (fast_enabled()) {
-    const int quads = (W + 3) / 4, rows = H < 8 ? H : 8, bands = (H + rows - 1) / rows;
-    const size_t tasks = (size_t)N * bands * quads;
-    int bx = (int)((tasks + tf::kT - 1) / tf::kT), cap = 4 * num_sms() / C;
-    cap = cap < 1 ? 1 : cap;
-    bx = bx > cap ? cap : bx;
-    float* part = nullptr;
-    if (int rc = partial_workspace((size_t)bx * C * 9, (cudaStream_t)stream, &part)) return rc;
-    tf::dw3_wgrad_kernel<<<dim3(bx, C), tf::kT, 0, (cudaStream_t)stream>>>(x, dy, part, N, C, H, W, quads, rows);
-    TR_CHECK(cudaGetLastError());
-    tf::reduce_partials_kernel<<<(C * 9 + tf::kT - 1) / tf::kT, tf::kT, 0, (cudaStream_t)stream>>>(part, bx, C * 9, scale, dw);
-  } else {
-    dw_wgrad_kernel<<<dim3(C, 9), kT, 0, (cudaStream_t)stream>>>(x, dy, dw, N, C, H, W, scale);
-  }
+  const int quads = (W + 3) / 4, rows = H < 8 ? H : 8, bands = (H + rows - 1) / rows;
+  const size_t tasks = (size_t)N * bands * quads;
+  int bx = (int)((tasks + tf::kT - 1) / tf::kT), cap = 4 * num_sms() / C;
+  cap = cap < 1 ? 1 : cap;
+  bx = bx > cap ? cap : bx;
+  float* part = nullptr;
+  if (int rc = partial_workspace((size_t)bx * C * 9, (cudaStream_t)stream, &part)) return rc;
+  tf::dw3_wgrad_kernel<<<dim3(bx, C), tf::kT, 0, (cudaStream_t)stream>>>(x, dy, part, N, C, H, W, quads, rows);
+  TR_CHECK(cudaGetLastError());
+  tf::reduce_partials_kernel<<<(C * 9 + tf::kT - 1) / tf::kT, tf::kT, 0, (cudaStream_t)stream>>>(part, bx, C * 9, scale, dw);
   TR_CHECK(cudaGetLastError());
   return CSNET_OK;
 }
@@ -758,33 +667,31 @@ int csnet_train_mix_fwd(float* dst, int32_t N, int32_t C, int32_t H, int32_t W, 
   csnet::MixArgs A{};
   A.dst = dst; A.bias = nullptr; A.slope = nullptr; A.dtype = CSNET_F32; A.C = C; A.H = H; A.W = W; A.n_paths = n_paths;
   for (int p = 0; p < n_paths; ++p) A.p[p] = to_path(paths[p]);
-  if (fast_enabled()) {
-    // every conv path dense with one kernel size, every other path a bilinear resample-add: the register-tiled kernel
-    tf::ConvArgs F{};
-    F.dst = dst; F.N = N; F.C = C; F.H = H; F.W = W; F.ksize = 1;
-    bool ok = conv_tile_geometry(F);
-    int ks = 0;
-    for (int p = 0; p < n_paths && ok; ++p) {
-      const csnet::MixPath& P = A.p[p];
-      if (P.ksize == 0) {
-        if (F.n_rs >= tf::kMaxRs || P.up < 2 || P.pre_avg || P.pool != 1 || P.H * P.up != H || P.W * P.up != W) { ok = false; break; }
-        tf::RsPath& Q = F.rs[F.n_rs++];
-        Q.src = reinterpret_cast<const float*>(P.src); Q.Cs = P.C; Q.c0 = P.c0; Q.Hs = P.H; Q.Ws = P.W; Q.up = P.up; Q.cout0 = P.cout0; Q.cout = P.cout;
-      } else {
-        if (F.n_conv >= tf::kMaxConv || !dense_conv_path(P, H, W) || (ks && ks != P.ksize)) { ok = false; break; }
-        ks = P.ksize;
-        tf::ConvPath& Q = F.p[F.n_conv++];
-        Q.src = reinterpret_cast<const float*>(P.src); Q.w = P.w; Q.Cs = P.C; Q.c0 = P.c0; Q.cin = P.cin; Q.cout0 = P.cout0; Q.cout = P.cout; Q.dil = P.dil;
-      }
+  // every conv path dense with one kernel size, every other path a bilinear resample-add: the register-tiled kernel
+  tf::ConvArgs F{};
+  F.dst = dst; F.N = N; F.C = C; F.H = H; F.W = W; F.ksize = 1;
+  bool ok = conv_tile_geometry(F);
+  int ks = 0;
+  for (int p = 0; p < n_paths && ok; ++p) {
+    const csnet::MixPath& P = A.p[p];
+    if (P.ksize == 0) {
+      if (F.n_rs >= tf::kMaxRs || P.up < 2 || P.pre_avg || P.pool != 1 || P.H * P.up != H || P.W * P.up != W) { ok = false; break; }
+      tf::RsPath& Q = F.rs[F.n_rs++];
+      Q.src = reinterpret_cast<const float*>(P.src); Q.Cs = P.C; Q.c0 = P.c0; Q.Hs = P.H; Q.Ws = P.W; Q.up = P.up; Q.cout0 = P.cout0; Q.cout = P.cout;
+    } else {
+      if (F.n_conv >= tf::kMaxConv || !dense_conv_path(P, H, W) || (ks && ks != P.ksize)) { ok = false; break; }
+      ks = P.ksize;
+      tf::ConvPath& Q = F.p[F.n_conv++];
+      Q.src = reinterpret_cast<const float*>(P.src); Q.w = P.w; Q.Cs = P.C; Q.c0 = P.c0; Q.cin = P.cin; Q.cout0 = P.cout0; Q.cout = P.cout; Q.dil = P.dil;
     }
-    if (ok) {
-      F.ksize = ks ? ks : 1;
-      for (int i = 0; i < F.n_conv && ok; ++i) ok = conv_path_geometry(F.p[i], F);
-    }
-    if (ok) {
-      const int rc = launch_conv(F, (cudaStream_t)stream);
-      if (rc != kNotHandled) return rc;
-    }
+  }
+  if (ok) {
+    F.ksize = ks ? ks : 1;
+    for (int i = 0; i < F.n_conv && ok; ++i) ok = conv_path_geometry(F.p[i], F);
+  }
+  if (ok) {
+    const int rc = launch_conv(F, (cudaStream_t)stream);
+    if (rc != kNotHandled) return rc;
   }
   tr_mix_fwd_kernel<<<dim3((H * W + kT - 1) / kT, (C + csnet::kMixCT - 1) / csnet::kMixCT, N), kT, 0, (cudaStream_t)stream>>>(A);
   TR_CHECK(cudaGetLastError());
@@ -794,7 +701,7 @@ int csnet_train_mix_fwd(float* dst, int32_t N, int32_t C, int32_t H, int32_t W, 
 int csnet_train_mix_dgrad(const float* ddst, int32_t N, int32_t C, int32_t H, int32_t W, const csnet_train_path* path, float* dsrc, void* stream) {
   const csnet::MixPath P = to_path(*path);
   if (P.pre_avg > 2 || P.up > 1 && P.ksize > 0) { t_err = "csnet_train_mix_dgrad: down-sample factors > 2 / input-side up-sampling are inference-only"; return CSNET_E_UNSUPPORTED; }
-  if (fast_enabled() && (size_t)N * P.cin * P.H * P.W < (1ull << 32) && P.ksize == 0 && (P.up == 2 || P.up == 4) && !P.pre_avg && P.pool == 1 && P.H * P.up == H && P.W * P.up == W) {
+  if ((size_t)N * P.cin * P.H * P.W < (1ull << 32) && P.ksize == 0 && (P.up == 2 || P.up == 4) && !P.pre_avg && P.pool == 1 && P.H * P.up == H && P.W * P.up == W) {
     const size_t total = (size_t)N * P.cin * P.H * P.W;
     const unsigned blocks = (unsigned)((total + tf::kT - 1) / tf::kT);
     if (P.up == 2) tf::resample_bwd_kernel<2><<<blocks, tf::kT, 0, (cudaStream_t)stream>>>(ddst, N, C, H, W, P.cout0, P.cin, P.H, P.W, dsrc);
@@ -802,7 +709,7 @@ int csnet_train_mix_dgrad(const float* ddst, int32_t N, int32_t C, int32_t H, in
     TR_CHECK(cudaGetLastError());
     return CSNET_OK;
   }
-  if (fast_enabled() && dense_conv_path(P, H, W)) {
+  if (dense_conv_path(P, H, W)) {
     tf::ConvArgs F{};
     F.dst = dsrc; F.N = N; F.C = P.cin; F.H = H; F.W = W; F.ksize = P.ksize; F.transposed = 1; F.n_conv = 1;
     tf::ConvPath& Q = F.p[0];
@@ -822,7 +729,7 @@ int csnet_train_mix_wgrad(const float* ddst, int32_t N, int32_t C, int32_t H, in
   if (P.ksize == 0) { t_err = "csnet_train_mix_wgrad: resample paths have no weights"; return CSNET_E_INVALID; }
   if (P.pre_avg > 2 || P.up > 1) { t_err = "csnet_train_mix_wgrad: down-sample factors > 2 / input-side up-sampling are inference-only"; return CSNET_E_UNSUPPORTED; }
   const int kk = P.ksize * P.ksize;
-  if (fast_enabled() && dense_conv_path(P, H, W) && (P.ksize == 3 || (P.ksize == 1 && P.dil == 1))) {
+  if (dense_conv_path(P, H, W) && (P.ksize == 3 || (P.ksize == 1 && P.dil == 1))) {
     const int form = P.ksize == 1 ? 1 : (P.dil == 1 ? 3 : 0);    // template argument of conv_wgrad_kernel
     tf::WgradArgs G{};
     G.in = reinterpret_cast<const float*>(P.src); G.dd = ddst; G.N = N; G.Cs = P.C; G.c0 = P.c0; G.cin = P.cin; G.Cd = C; G.cout0 = P.cout0;
@@ -890,8 +797,7 @@ int csnet_train_pool_fwd(const float* src, int32_t N, int32_t Cs, int32_t c0, in
   const int f = (pre_avg ? 2 : 1) * pool;
   const size_t total = (size_t)N * cin * (Hs / f) * (Ws / f);
   if (total == 0) return CSNET_OK;
-  static const bool pool2 = [] { const char* e = getenv("CSNET_POOL2"); return !(e && e[0] == '0'); }();
-  if (pool2 && !pre_avg && pool == 2 && Ws % 4 == 0 && Hs % 2 == 0 && total < (1ull << 31))
+  if (!pre_avg && pool == 2 && Ws % 4 == 0 && Hs % 2 == 0 && total < (1ull << 31))
     tf::pool2_fwd_kernel<<<(unsigned)((total / 2 + tf::kT - 1) / tf::kT), tf::kT, 0, (cudaStream_t)stream>>>(src, N, Cs, c0, cin, Hs, Ws, dst, idx);
   else
     tf::pool_fwd_kernel<<<(unsigned)((total + tf::kT - 1) / tf::kT), tf::kT, 0, (cudaStream_t)stream>>>(src, N, Cs, c0, cin, Hs, Ws, pre_avg, pool, dst, idx);

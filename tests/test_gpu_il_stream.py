@@ -1,6 +1,7 @@
 """The streaming ILBlock kernel (csrc/il_stream.cuh: TMA operand tiles, wgmma GEMM with register accumulators, register-resident
 depthwise tail) against the generic ops, the tiled kernel and the oracle.  CSNET_ILS / CSNET_ILS_MIN_CHUNKS / CSNET_ILS_NS are
 read when a plan is created, so a test can pin which kernel runs an ILBLOCK op."""
+import collections
 import os
 
 import numpy as np
@@ -133,3 +134,31 @@ def test_msblock_direct_kernel_matches_generic_ops(tag, hw):
             assert (a - b).abs().max().item() <= 4e-3 * max(1.0, b.abs().max().item()), name
             n += 1
     assert n >= 2
+
+
+def _kernel_counts(dtype, max_batch):
+    """(ops per kernel name, launches per forward) of the csnet-L-x2 plan at 224x224 that bench.py and smoke() run."""
+    cfg, sd = fixtures.checkpoint("csnet-L-x2")
+    p = runtime.Plan(compiler.compile_csnet(cfg, sd, 224, 224, dtype), max_batch=max_batch)
+    try:
+        return dict(collections.Counter(p.op_kernel(i) for i in range(len(p.prog.ops)))), p.launches
+    finally:
+        p.close()
+
+
+# Recorded on an H100 80GB HBM3 (132 SMs) with none of the CSNET_* switches set.
+EXPECTED_KERNELS = {
+    ("fp16", 256): ({"il_stream_kernel (TMA + wgmma)": 7, "il_block_kernel (mma.sync, tiled)": 5, "mix_stream_kernel (TMA + wgmma)": 8,
+                     "mix_tc_kernel (mma.sync)": 15, "msd_kernel (ms_direct.cuh, FP32 pipe)": 2, "pool2 / upsample / resample kernels": 15,
+                     "dw kernels": 22}, 81),
+    ("fp16", 2): ({"il_block_kernel (mma.sync, tiled)": 12, "mix_tc_kernel (mma.sync)": 23, "msd_kernel (ms_direct.cuh, FP32 pipe)": 2,
+                   "pool2 / upsample / resample kernels": 15, "dw kernels": 22}, 81),
+    ("fp32", 256): ({"mix_generic_kernel": 61, "pool2 / upsample / resample kernels": 1, "dw kernels": 66}, 128),
+}
+
+
+@pytest.mark.parametrize("dtype,max_batch", list(EXPECTED_KERNELS))
+def test_kernel_selection_of_the_bench_plans(dtype, max_batch):
+    """Which kernel runs each op is fixed when the plan is created (max_batch and the SM count pick the streaming or the
+    tiled / graph-replayed side): pin it for the bench configuration, its small-batch form and the fp32 program."""
+    assert _kernel_counts(dtype, max_batch) == EXPECTED_KERNELS[(dtype, max_batch)]
