@@ -47,7 +47,7 @@ def _padded_region(n: int) -> int:
 
 
 def il_block_fits(Chi, Cli, Cho, Clo) -> bool:
-    """Mirror of make_il() in csrc/plan.cu: K = Chi + Cli must fit the register-resident B fragments (<= 64) and the
+    """Mirror of plan_il() in csrc/plan.cu: K = Chi + Cli must fit the register-resident B fragments (<= 64) and the
     smallest candidate tile (8 x 16) must fit 227 KB of shared memory."""
     K8, MH16, ML16 = _ru(Chi + Cli, 8), _ru(Cho, 16), (_ru(Clo, 16) if Clo else 0)
     if K8 > 64:

@@ -180,6 +180,24 @@ size_t tc_smem_bytes(const TcChoice& c) {
   return ((size_t)c.kc * c.xs_halves + (size_t)c.kk * c.mt * 16 * (c.kc + 8)) * 2;
 }
 
+using IlKernel = void (*)(csnet::IlArgs);
+using TcKernel = void (*)(csnet::MixArgs, csnet::TcGeom);
+
+// How launch_op() runs one op: the kernel chosen for it and every kernel argument that does not depend on the call, planned
+// when the plan is created (the epilogue tables when the blob is set).  launch_op() binds the activation addresses, the batch
+// and the tensor maps.  A streaming record stays zero when its kernel cannot take the op.
+struct OpLaunch {
+  Kern kern = Kern::MixGeneric;
+  TcChoice tc;                                    // MIX ops: mt > 0 if the tensor-core kernel can take the op
+  csnet::MsArgs ms{};                             // MIX ops: the streaming kernel's arguments (n_in > 0 if it can take the op)
+  csnet::IlArgs il{};                             // ILBLOCK ops: the tiled kernel's arguments with the tile chosen
+  csnet::IlsArgs ils{};                           // ILBLOCK ops: the streaming kernel's arguments (ns > 0 if it can take the op)
+  size_t smem = 0;                                // MixTc / IlBlock: dynamic shared memory of a launch
+  TcKernel tc_fn = nullptr;                       // MixTc: the mix_tc_kernel instantiation
+  IlKernel il_fn = nullptr;                       // IlBlock: the il_block_kernel instantiation
+  uint16_t* w16[CSNET_MAX_PATHS] = {};            // MixTc: per path, packed 16-bit weights (device)
+};
+
 struct csnet_plan {
   int device = 0;
   int max_batch = 0;
@@ -190,17 +208,12 @@ struct csnet_plan {
   char* arena = nullptr;
   int64_t arena_per_image = 0;   // bytes
   int n_ext = 0;
-  size_t il_smem_max = 0;
-  std::vector<size_t> op_smem;
-  std::vector<TcChoice> op_tc;
-  std::vector<std::vector<uint16_t*>> op_w16;     // per tensor-core MIX op, per path: packed 16-bit weights (device)
-  std::vector<float> h_blob;                      // host copy of the blob (epilogue tables of the streaming ILBlock kernel)
+  std::vector<OpLaunch> launch;                   // per op
   // small-batch replay: the whole op list captured once per batch size into a CUDA graph over plan-owned input / output staging
   // (CSNet/test.py calls the model one image at a time: ~80 launches per forward are launch-bound there)
   struct GraphSlot { cudaGraphExec_t exec = nullptr; void* in = nullptr; void* out = nullptr; size_t in_bytes = 0, out_bytes = 0; };
   std::vector<GraphSlot> graphs;                  // index = batch size
   cudaStream_t cap_stream = nullptr;
-  std::vector<Kern> op_kern;                      // per op: the kernel launch_op() runs
   bool ms_enabled = true;                         // CSNET_MS=0 at plan creation: mix_tc / generic kernels only
   int num_sms = 132;
   int ils_force_ns = 0;                           // CSNET_ILS_NS=k: force k column strips (0: automatic)
@@ -406,18 +419,15 @@ EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
-// Fill the kernel arguments of a fused ILBlock op and pick its tile; false if no tile fits shared memory.
-bool make_il(const csnet_plan& P, const csnet_op_desc& op, int N, const void* const* ext, csnet::IlArgs* out) {
+// Kernel arguments of a fused ILBlock op on the tiled kernel, but for the activation addresses (bound at launch), and its
+// tile; false if no tile fits shared memory.
+bool plan_il(const csnet_plan& P, const csnet_op_desc& op, csnet::IlArgs* out) {
   csnet::IlArgs A{};
   const csnet_tensor_desc &Xh = P.tensors[op.paths[0].src], &Xl = P.tensors[op.paths[1].src], &Yh = P.tensors[op.dst];
-  A.xh = P.tensor_ptr(op.paths[0].src, N, ext);
-  A.xl = P.tensor_ptr(op.paths[1].src, N, ext);
-  A.yh = P.tensor_ptr(op.dst, N, ext);
-  A.yl = op.dst2 >= 0 ? P.tensor_ptr(op.dst2, N, ext) : nullptr;
   A.H = Yh.H; A.W = Yh.W;
   A.Chi = Xh.C; A.Cli = Xl.C; A.Cho = Yh.C; A.Clo = op.dst2 >= 0 ? P.tensors[op.dst2].C : 0;
   A.first = op.paths[0].ksize == 3;
-  if (A.first) { A.Chi = Xh.C * 9; A.Cli = 0; A.xl = nullptr; }   // im2col rows of the image; no lo input tensor
+  if (A.first) { A.Chi = Xh.C * 9; A.Cli = 0; }   // im2col rows of the image; no lo input tensor
   auto f = [&](int e) { return op.ext_off[e] >= 0 ? P.blob + op.ext_off[e] : nullptr; };
   A.wh = reinterpret_cast<const uint32_t*>(f(0));
   A.wl = reinterpret_cast<const uint32_t*>(f(1));
@@ -482,10 +492,11 @@ bool encode_image_map(CUtensorMap* tm, const void* base, int N, int C, int H, in
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// Geometry of the streaming ILBlock kernel for an op; false if the op does not qualify (the tiled kernel runs it).
+// Kernel arguments of an ILBlock op on the streaming kernel, but for the outputs, the batch and the epilogue tables; false if
+// the op does not qualify (the tiled kernel runs it).  The parameter pointers are the tiled kernel's (`il`).
 // Picks the column-strip split: the fewest strips that fit the thread / shared-memory limits.
-bool make_ils(const csnet_plan& P, const csnet_op_desc& op, csnet::IlsArgs* out) {
-  if (!P.ils_enabled || op.kind != CSNET_OP_ILBLOCK || encode_tiled_fn() == nullptr) return false;
+bool plan_ils(const csnet_plan& P, const csnet_op_desc& op, const csnet::IlArgs& il, csnet::IlsArgs* out) {
+  if (!P.ils_enabled || encode_tiled_fn() == nullptr) return false;
   const csnet_tensor_desc &Xh = P.tensors[op.paths[0].src], &Xl = P.tensors[op.paths[1].src], &Yh = P.tensors[op.dst];
   if (Yh.dtype != CSNET_F16) return false;
   const bool stem = op.paths[0].ksize == 3;                              // stem form: 3x3 convs of the fp32 image (im2col K = 9 Ci)
@@ -545,13 +556,9 @@ bool make_ils(const csnet_plan& P, const csnet_op_desc& op, csnet::IlsArgs* out)
     if (!found || cost < best_cost) { best = T; best_cost = cost; found = true; }
   }
   if (!found) return false;
-  A = best;
-  if ((int64_t)P.h_blob.size() == P.blob_floats) {       // (a geometry query before the blob exists leaves the tables zero)
-    auto f = [&](int e) { return op.ext_off[e] >= 0 ? P.h_blob.data() + op.ext_off[e] : nullptr; };
-    for (int c = 0; c < A.Cho; ++c) { A.bias_h[c] = f(2)[c]; A.sm1_h[c] = f(3)[c] - 1.f; }
-    for (int c = 0; c < A.Clo; ++c) { A.bias_l[c] = f(4)[c]; A.sm1_l[c] = f(5)[c] - 1.f; }
-  }
-  *out = A;
+  best.wh = il.wh; best.wl = il.wl;
+  best.dw1h = il.dw1h; best.dw1l = il.dw1l; best.dw2h = il.dw2h; best.dw2l = il.dw2l;
+  *out = best;
   return true;
 }
 
@@ -572,9 +579,10 @@ bool is_msd(const csnet_plan& P, const csnet_op_desc& op) {
   return true;
 }
 
-// Kernel arguments of the streaming 1x1 MIX kernel for an op; false if the op does not qualify.
-bool make_ms(const csnet_plan& P, const csnet_op_desc& op, int N, const void* const* ext, csnet::MsArgs* out, CUtensorMap* maps) {
-  if (!P.ms_enabled || (op.kind != CSNET_OP_MIX && op.kind != CSNET_OP_MIXPROJ) || encode_tiled_fn() == nullptr) return false;
+// Kernel arguments of a MIX op on the streaming 1x1 MIX kernel, but for the activation addresses, the batch and the epilogue
+// tables; false if the op does not qualify.
+bool plan_ms(const csnet_plan& P, const csnet_op_desc& op, csnet::MsArgs* out) {
+  if (!P.ms_enabled || encode_tiled_fn() == nullptr) return false;
   if (op.kind == CSNET_OP_MIX && op.ext_off[23] == 1) return false;      // the compiler's veto of 16-bit weights
   const csnet_tensor_desc& D = P.tensors[op.dst];
   csnet::MsArgs A{};
@@ -583,7 +591,7 @@ bool make_ms(const csnet_plan& P, const csnet_op_desc& op, int N, const void* co
   if (A.C > csnet::kMsMaxC || D.W % 8 || D.H % csnet::kMsRows) return false;
   if (A.has_proj ? D.dtype != CSNET_F32 : D.dtype == CSNET_BF16) return false;
   A.dst_f32 = D.dtype == CSNET_F32;
-  A.H = D.H; A.W = D.W; A.N = N; A.G = D.W / 8; A.NN = round_up(A.C, 16);
+  A.H = D.H; A.W = D.W; A.G = D.W / 8; A.NN = round_up(A.C, 16);
   int off = 0;
   auto r128 = [](int v) { return (v + 127) / 128 * 128; };
   for (int p = 0; p < op.n_paths; ++p) {
@@ -592,7 +600,6 @@ bool make_ms(const csnet_plan& P, const csnet_op_desc& op, int N, const void* co
     if (q.ksize == 0) {
       if (A.n_rs >= csnet::kMsMaxRs || q.up < 2 || q.pool != 1 || q.pre_avg || S.H * q.up != D.H || S.W * q.up != D.W || S.dtype != CSNET_F32 || q.cout0 != 0) return false;
       const int j = A.n_rs++;
-      A.rsrc[j] = ext || S.external < 0 ? P.tensor_ptr(q.src, N, ext) : nullptr;
       A.r_dtype[j] = S.dtype; A.r_up[j] = q.up; A.r_H[j] = S.H; A.r_W[j] = S.W; A.r_C[j] = S.C; A.r_c0[j] = q.c0; A.r_cout0[j] = q.cout0; A.r_n[j] = q.cout;
       continue;
     }
@@ -609,8 +616,7 @@ bool make_ms(const csnet_plan& P, const csnet_op_desc& op, int N, const void* co
     A.in_off[i] = off;
     A.copy_bytes[i] = r128(trows * A.G * A.S[i] * 16);
     off += (k3 ? 3 : 1) * A.copy_bytes[i];
-    if (maps && !encode_group_map(&maps[i], P.tensor_ptr(q.src, N, ext), N, S.C, S.H, S.W, A.S[i], A.G, trows)) return false;
-    if (q.c0 != 0) return false;                                            // (a channel-sliced source would need a c0 coordinate)
+    if (q.c0 != 0) return false;                                           // (a channel-sliced source would need a c0 coordinate)
   }
   if (A.n_in == 0) return false;
   A.stage_bytes = off;
@@ -618,7 +624,6 @@ bool make_ms(const csnet_plan& P, const csnet_op_desc& op, int N, const void* co
   for (int i = 0; i < A.n_in; ++i) A.tx_bytes += (csnet::kMsRows + (A.k3 ? 2 : 0)) * A.G * A.S[i] * 16;
   A.nb = (csnet::kMsRows * A.G + 7) / 8;
   A.cpi = D.H / csnet::kMsRows;
-  A.total_chunks = N * A.cpi;
   int wb = 0;
   const int taps = A.k3 ? 9 : 1;
   for (int i = 0; i < A.n_in; ++i) wb += r128(taps * A.NN * A.K16[i] * 2);
@@ -633,36 +638,17 @@ bool make_ms(const csnet_plan& P, const csnet_op_desc& op, int N, const void* co
   A.off_tab = o; o += 1280;
   A.smem_bytes = o + 128;
   A.has_slope = op.slope_off >= 0;
-  if ((int64_t)P.h_blob.size() == P.blob_floats) {
-    for (int c = 0; c < A.C; ++c) {
-      A.bias[c] = op.bias_off >= 0 ? P.h_blob[op.bias_off + c] : 0.f;
-      A.sm1[c] = op.slope_off >= 0 ? P.h_blob[op.slope_off + c] - 1.f : 0.f;
-      A.proj[c] = A.has_proj ? P.h_blob[op.ext_off[0] + c] : 0.f;
-    }
-    A.proj_b = A.has_proj && op.ext_off[1] >= 0 ? P.h_blob[op.ext_off[1]] : 0.f;
-  }
-  A.dst = ext || D.external < 0 ? P.tensor_ptr(op.dst, N, ext) : nullptr;
   *out = A;
   return true;
 }
 
+// The il_block_kernel instantiation of a tile (plan_il's candidates).
 template <typename T>
-void launch_il_t(const csnet::IlArgs& A, dim3 grid, size_t smem, cudaStream_t st) {
-  if (A.TH == 32) csnet::il_block_kernel<T, 32, 32><<<grid, csnet::kIlThreads, smem, st>>>(A);
-  else if (A.TH == 28) csnet::il_block_kernel<T, 28, 32><<<grid, csnet::kIlThreads, smem, st>>>(A);
-  else if (A.TH == 16 && A.TW == 64) csnet::il_block_kernel<T, 16, 64><<<grid, csnet::kIlThreads, smem, st>>>(A);
-  else if (A.TH == 16) csnet::il_block_kernel<T, 16, 32><<<grid, csnet::kIlThreads, smem, st>>>(A);
-  else csnet::il_block_kernel<T, 8, 16><<<grid, csnet::kIlThreads, smem, st>>>(A);
-}
-
-template <typename T>
-cudaError_t set_il_smem_t(int bytes) {
-  cudaError_t e = cudaFuncSetAttribute(csnet::il_block_kernel<T, 32, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::il_block_kernel<T, 28, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::il_block_kernel<T, 16, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::il_block_kernel<T, 16, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::il_block_kernel<T, 8, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  return e;
+IlKernel il_kernel(const csnet::IlArgs& A) {
+  if (A.TH == 32) return csnet::il_block_kernel<T, 32, 32>;
+  if (A.TH == 28) return csnet::il_block_kernel<T, 28, 32>;
+  if (A.TH == 16) return A.TW == 64 ? csnet::il_block_kernel<T, 16, 64> : csnet::il_block_kernel<T, 16, 32>;
+  return csnet::il_block_kernel<T, 8, 16>;
 }
 
 // Can this MIX op run on the tensor-core kernel (mix_tc.cuh)?  Needs 16-bit operands somewhere, stride-1 conv
@@ -701,18 +687,14 @@ TcChoice choose_tc(const csnet_plan& P, const csnet_op_desc& op) {
   return c;
 }
 
-// The kernel that runs op i; the first one in this order that takes the op wins.  Every input is fixed when the plan is
-// created (the op, its tensors, op_tc, max_batch, the SM count, the switches), never by the batch of a call: every sub-batch
-// of a plan runs the same kernels, bit for bit.
-Kern choose_kernel(const csnet_plan& P, size_t i) {
-  const csnet_op_desc& op = P.ops[i];
+// The kernel that runs an op; the first one in this order that takes the op wins.  Every input is fixed when the plan is
+// created (the op, its tensors, its planned record R, max_batch, the SM count, the switches), never by the batch of a call:
+// every sub-batch of a plan runs the same kernels, bit for bit.
+Kern choose_kernel(const csnet_plan& P, const csnet_op_desc& op, const OpLaunch& R) {
   const csnet_tensor_desc& D = P.tensors[op.dst];
-  csnet::MsArgs M;
-  csnet::IlsArgs S;
   if (is_msd(P, op)) return Kern::Msd;
-  if (make_ms(P, op, 1, nullptr, &M, nullptr) && (int64_t)P.max_batch * (D.H / csnet::kMsRows) >= (int64_t)2 * P.num_sms)
-    return Kern::MixStream;
-  if ((op.kind == CSNET_OP_MIX || op.kind == CSNET_OP_MIXPROJ) && P.op_tc[i].mt > 0) return Kern::MixTc;
+  if (R.ms.n_in > 0 && (int64_t)P.max_batch * (D.H / csnet::kMsRows) >= (int64_t)2 * P.num_sms) return Kern::MixStream;
+  if ((op.kind == CSNET_OP_MIX || op.kind == CSNET_OP_MIXPROJ) && R.tc.mt > 0) return Kern::MixTc;
   if (op.kind == CSNET_OP_MIX && op.n_paths == 1 && op.paths[0].ksize == 0 && op.paths[0].cout0 == 0 && op.paths[0].cout == D.C) {
     const csnet_path_desc& q = op.paths[0];                    // a pure resample
     const csnet_tensor_desc& Sq = P.tensors[q.src];
@@ -725,39 +707,91 @@ Kern choose_kernel(const csnet_plan& P, size_t i) {
   if (op.kind == CSNET_OP_MIX) return Kern::MixGeneric;
   if (op.kind == CSNET_OP_GN) return Kern::Gn;
   if (op.kind == CSNET_OP_ILBLOCK)
-    return make_ils(P, op, &S) && (int64_t)P.max_batch * (D.H / 4) >= (int64_t)P.ils_min_chunks ? Kern::IlStream : Kern::IlBlock;
+    return R.ils.ns > 0 && (int64_t)P.max_batch * (D.H / 4) >= (int64_t)P.ils_min_chunks ? Kern::IlStream : Kern::IlBlock;
   const csnet_tensor_desc& Sd = P.tensors[op.paths[0].src];
   return op.ext_off[23] != 1 && Sd.dtype == D.dtype && D.dtype != CSNET_F32 && D.W % 4 == 0 ? Kern::DwFast : Kern::DwGeneric;
 }
 
+// The mix_tc_kernel instantiation of a choice (choose_tc gives rows 4 only with mt 1, rows 2 only with mt 2).
 template <typename T>
-void launch_mix_tc_t(int mt, dim3 grid, size_t smem, cudaStream_t st, const csnet::MixArgs& A, const csnet::TcGeom& G) {
-  if (G.rows == 4) { csnet::mix_tc_kernel<T, 1, 4><<<grid, csnet::kTcThreads, smem, st>>>(A, G); return; }
-  if (G.rows == 2) { csnet::mix_tc_kernel<T, 2, 2><<<grid, csnet::kTcThreads, smem, st>>>(A, G); return; }
-  switch (mt) {
-    case 1: csnet::mix_tc_kernel<T, 1><<<grid, csnet::kTcThreads, smem, st>>>(A, G); break;
-    case 2: csnet::mix_tc_kernel<T, 2><<<grid, csnet::kTcThreads, smem, st>>>(A, G); break;
-    case 3: csnet::mix_tc_kernel<T, 3><<<grid, csnet::kTcThreads, smem, st>>>(A, G); break;
-    case 4: csnet::mix_tc_kernel<T, 4><<<grid, csnet::kTcThreads, smem, st>>>(A, G); break;
-    default: csnet::mix_tc_kernel<T, 5><<<grid, csnet::kTcThreads, smem, st>>>(A, G); break;
+TcKernel tc_kernel(const TcChoice& c) {
+  if (c.rows == 4) return csnet::mix_tc_kernel<T, 1, 4>;
+  if (c.rows == 2) return csnet::mix_tc_kernel<T, 2, 2>;
+  switch (c.mt) {
+    case 1: return csnet::mix_tc_kernel<T, 1>;
+    case 2: return csnet::mix_tc_kernel<T, 2>;
+    case 3: return csnet::mix_tc_kernel<T, 3>;
+    case 4: return csnet::mix_tc_kernel<T, 4>;
+    default: return csnet::mix_tc_kernel<T, 5>;
   }
 }
 
-void launch_mix_tc(const TcChoice& c, dim3 grid, size_t smem, cudaStream_t st, const csnet::MixArgs& A, const csnet::TcGeom& G) {
-  if (c.dtype == CSNET_F16) launch_mix_tc_t<__half>(c.mt, grid, smem, st, A, G);
-  else launch_mix_tc_t<__nv_bfloat16>(c.mt, grid, smem, st, A, G);
-}
+// The dynamic shared memory a kernel may opt into on sm_90 (227 KB less its static shared memory; these kernels have none).
+// Each kernel is given all of it, not what one plan needs: the attribute belongs to the kernel, so a plan created later must
+// not lower the limit an existing plan relies on.
+constexpr int kSmemOptIn = 227 * 1024;
 
-template <typename T>
-cudaError_t set_tc_smem_t(int bytes) {
-  cudaError_t e = cudaFuncSetAttribute(csnet::mix_tc_kernel<T, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::mix_tc_kernel<T, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::mix_tc_kernel<T, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::mix_tc_kernel<T, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::mix_tc_kernel<T, 5>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::mix_tc_kernel<T, 1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::mix_tc_kernel<T, 2, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  return e;
+const char* const kKernNames[] = {
+    "msd_kernel (ms_direct.cuh, FP32 pipe)", "mix_stream_kernel (TMA + wgmma)", "mix_tc_kernel (mma.sync)",
+    "pool2 / upsample / resample kernels", "pool2 / upsample / resample kernels", "pool2 / upsample / resample kernels",
+    "mix_generic_kernel", "gn kernels", "il_stream_kernel (TMA + wgmma)", "il_block_kernel (mma.sync, tiled)", "dw kernels", "dw kernels"};
+static_assert(sizeof kKernNames / sizeof kKernNames[0] == (size_t)Kern::DwGeneric + 1, "one name per Kern");
+
+// Plan op i: choose its kernel and fill its launch record (kernel, static arguments, packed-weight buffers), and let the
+// kernel use the shared memory it needs.
+int plan_op(csnet_plan& P, size_t i) {
+  const csnet_op_desc& op = P.ops[i];
+  OpLaunch& R = P.launch[i];
+  if (op.kind == CSNET_OP_MIX || op.kind == CSNET_OP_MIXPROJ) {
+    R.tc = choose_tc(P, op);
+    if (tc_smem_bytes(R.tc) > 200 * 1024) R.tc = TcChoice();
+    if (op.kind == CSNET_OP_MIXPROJ && R.tc.mt == 0)
+      return fail(CSNET_E_UNSUPPORTED, "MIXPROJ op does not qualify for the tensor-core kernel (16-bit sources, stride 1, pad <= limit)");
+    plan_ms(P, op, &R.ms);
+  } else if (op.kind == CSNET_OP_ILBLOCK) {
+    if (!plan_il(P, op, &R.il)) return fail(CSNET_E_UNSUPPORTED, "ILBLOCK op does not fit shared memory");
+    plan_ils(P, op, R.il, &R.ils);
+  }
+  R.kern = choose_kernel(P, op, R);
+  cudaError_t e = cudaSuccess;
+  switch (R.kern) {
+    case Kern::MixStream:
+      e = cudaFuncSetAttribute(csnet::mix_stream_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOptIn);
+      break;
+    case Kern::MixTc: {
+      const int C = mix_channels(P, op), slice = R.tc.mt * 16, m16t = (C + slice - 1) / slice * slice, WR = R.tc.kc + 8;
+      for (int p = 0; p < op.n_paths; ++p) {
+        const csnet_path_desc& q = op.paths[p];
+        if (q.ksize == 0) continue;
+        const size_t halves = (size_t)((q.cin + R.tc.kc - 1) / R.tc.kc) * q.ksize * q.ksize * m16t * WR;
+        e = cudaMalloc(&R.w16[p], halves * 2);
+        if (e != cudaSuccess) return fail(CSNET_E_NOMEM, std::string("cudaMalloc(packed weights): ") + cudaGetErrorString(e));
+      }
+      R.smem = tc_smem_bytes(R.tc);
+      R.tc_fn = R.tc.dtype == CSNET_F16 ? tc_kernel<__half>(R.tc) : tc_kernel<__nv_bfloat16>(R.tc);
+      e = cudaFuncSetAttribute(R.tc_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOptIn);
+      break;
+    }
+    case Kern::IlStream: {
+      const bool stem = R.ils.Ci > 0;
+      e = cudaFuncSetAttribute(stem ? csnet::il_stream_kernel<__half, true> : csnet::il_stream_kernel<__half, false>,
+                               cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOptIn);
+      // two CTAs of <= 113 KB share an SM only with the full shared-memory carve-out
+      if (e == cudaSuccess && !stem)
+        e = cudaFuncSetAttribute(csnet::il_stream_kernel<__half, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+      break;
+    }
+    case Kern::IlBlock:
+      R.smem = il_smem_of(R.il);
+      R.il_fn = P.tensors[op.dst].dtype == CSNET_F16 ? il_kernel<__half>(R.il) : il_kernel<__nv_bfloat16>(R.il);
+      e = cudaFuncSetAttribute(R.il_fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOptIn);
+      break;
+    default:
+      break;
+  }
+  if (e != cudaSuccess)
+    return fail(CSNET_E_CUDA, std::string("cudaFuncSetAttribute(") + kKernNames[(int)R.kern] + "): " + cudaGetErrorString(e));
+  return CSNET_OK;
 }
 
 }  // namespace
@@ -816,50 +850,6 @@ int csnet_plan_create(csnet_plan** out, const csnet_tensor_desc* tensors, int32_
     e = cudaMalloc(&P->gn_stats, (size_t)max_batch * P->gn_groups_max * 2 * sizeof(float));
     if (e != cudaSuccess) return cleanup(CSNET_E_NOMEM, std::string("cudaMalloc(gn stats): ") + cudaGetErrorString(e));
   }
-  // dynamic shared memory each MIX op needs (weights of one cout tile)
-  P->op_smem.assign(P->ops.size(), 0);
-  P->op_tc.assign(P->ops.size(), TcChoice());
-  size_t tc_smem_max = 0;
-  for (size_t i = 0; i < P->ops.size(); ++i) {
-    if (P->ops[i].kind != CSNET_OP_MIX && P->ops[i].kind != CSNET_OP_MIXPROJ) continue;
-    P->op_tc[i] = choose_tc(*P, P->ops[i]);
-    if (P->op_tc[i].mt > 0 && tc_smem_bytes(P->op_tc[i]) <= 200 * 1024) {
-      P->op_smem[i] = tc_smem_bytes(P->op_tc[i]);
-      tc_smem_max = P->op_smem[i] > tc_smem_max ? P->op_smem[i] : tc_smem_max;
-      continue;
-    }
-    if (P->ops[i].kind == CSNET_OP_MIXPROJ)
-      return cleanup(CSNET_E_UNSUPPORTED, "MIXPROJ op does not qualify for the tensor-core kernel (16-bit sources, stride 1, pad <= limit)");
-    P->op_tc[i] = TcChoice();
-    P->op_smem[i] = 0;                                   // the generic kernel stages weights in static shared memory
-  }
-  P->op_w16.assign(P->ops.size(), std::vector<uint16_t*>());
-  for (size_t i = 0; i < P->ops.size(); ++i) {
-    const TcChoice& tc = P->op_tc[i];
-    if (tc.mt <= 0) continue;
-    const csnet_op_desc& op = P->ops[i];
-    const int C = mix_channels(*P, op), slice = tc.mt * 16, m16t = (C + slice - 1) / slice * slice, WR = tc.kc + 8;
-    P->op_w16[i].assign(op.n_paths, nullptr);
-    for (int p = 0; p < op.n_paths; ++p) {
-      const csnet_path_desc& q = op.paths[p];
-      if (q.ksize == 0) continue;
-      const size_t halves = (size_t)((q.cin + tc.kc - 1) / tc.kc) * q.ksize * q.ksize * m16t * WR;
-      e = cudaMalloc(&P->op_w16[i][p], halves * 2);
-      if (e != cudaSuccess) return cleanup(CSNET_E_NOMEM, std::string("cudaMalloc(packed weights): ") + cudaGetErrorString(e));
-    }
-  }
-  if (tc_smem_max > 48 * 1024) {
-    e = set_tc_smem_t<__half>((int)tc_smem_max);
-    if (e == cudaSuccess) e = set_tc_smem_t<__nv_bfloat16>((int)tc_smem_max);
-    if (e != cudaSuccess) return cleanup(CSNET_E_CUDA, std::string("cudaFuncSetAttribute(mix_tc): ") + cudaGetErrorString(e));
-  }
-  for (size_t i = 0; i < P->ops.size(); ++i) {
-    if (P->ops[i].kind != CSNET_OP_ILBLOCK) continue;
-    csnet::IlArgs A;
-    if (!make_il(*P, P->ops[i], 1, nullptr, &A)) return cleanup(CSNET_E_UNSUPPORTED, "ILBLOCK op does not fit shared memory");
-    P->op_smem[i] = il_smem_of(A);
-    P->il_smem_max = P->op_smem[i] > P->il_smem_max ? P->op_smem[i] : P->il_smem_max;
-  }
   {
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) == cudaSuccess && prop.multiProcessorCount > 0) P->num_sms = prop.multiProcessorCount;
@@ -871,29 +861,10 @@ int csnet_plan_create(csnet_plan** out, const csnet_tensor_desc* tensors, int32_
   if (const char* s = getenv("CSNET_ILS_NS")) P->ils_force_ns = atoi(s);
   P->ils_min_chunks = 4 * P->num_sms;
   if (const char* s = getenv("CSNET_ILS_MIN_CHUNKS")) P->ils_min_chunks = atoi(s);
-  P->op_kern.resize(P->ops.size());
-  bool any_ms = false, any_ils = false;
+  P->launch.resize(P->ops.size());
   for (size_t i = 0; i < P->ops.size(); ++i) {
-    P->op_kern[i] = choose_kernel(*P, i);
-    any_ms |= P->op_kern[i] == Kern::MixStream;
-    any_ils |= P->op_kern[i] == Kern::IlStream;
-  }
-  if (any_ms) {
-    e = cudaFuncSetAttribute(csnet::mix_stream_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) return cleanup(CSNET_E_CUDA, std::string("cudaFuncSetAttribute(mix_stream): ") + cudaGetErrorString(e));
-  }
-  if (any_ils) {
-    // always the architectural maximum: plans created later must not lower the limit an earlier plan relies on
-    e = cudaFuncSetAttribute(csnet::il_stream_kernel<__half, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::il_stream_kernel<__half, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    // two CTAs of <= 113 KB share an SM only with the full shared-memory carve-out
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(csnet::il_stream_kernel<__half, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    if (e != cudaSuccess) return cleanup(CSNET_E_CUDA, std::string("cudaFuncSetAttribute(il_stream): ") + cudaGetErrorString(e));
-  }
-  if (P->il_smem_max > 0) {
-    e = set_il_smem_t<__half>((int)P->il_smem_max);
-    if (e == cudaSuccess) e = set_il_smem_t<__nv_bfloat16>((int)P->il_smem_max);
-    if (e != cudaSuccess) return cleanup(CSNET_E_CUDA, std::string("cudaFuncSetAttribute(il_block): ") + cudaGetErrorString(e));
+    rc = plan_op(*P, i);
+    if (rc != CSNET_OK) { csnet_plan_destroy(P); return rc; }
   }
   *out = P;
   return CSNET_OK;
@@ -905,14 +876,33 @@ int csnet_plan_set_blob(csnet_plan* P, const float* host_blob, int64_t n, void* 
   if (!P || !host_blob || n != P->blob_floats) return fail(CSNET_E_INVALID, "csnet_plan_set_blob: size mismatch");
   DeviceGuard guard_(P->device);
   CU_CHECK(cudaMemcpyAsync(P->blob, host_blob, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, (cudaStream_t)stream));
-  P->h_blob.assign(host_blob, host_blob + n);
   drop_graphs(P);                                   // captured launches carry parameter tables of the old blob
+  // the streaming kernels take their bias / PReLU / projection epilogue tables in the kernel arguments
+  for (size_t i = 0; i < P->ops.size(); ++i) {
+    const csnet_op_desc& op = P->ops[i];
+    OpLaunch& R = P->launch[i];
+    if (R.kern == Kern::IlStream) {
+      csnet::IlsArgs& A = R.ils;
+      for (int c = 0; c < A.Cho; ++c) { A.bias_h[c] = host_blob[op.ext_off[2] + c]; A.sm1_h[c] = host_blob[op.ext_off[3] + c] - 1.f; }
+      for (int c = 0; c < A.Clo; ++c) { A.bias_l[c] = host_blob[op.ext_off[4] + c]; A.sm1_l[c] = host_blob[op.ext_off[5] + c] - 1.f; }
+    }
+    if (R.kern == Kern::MixStream) {
+      csnet::MsArgs& A = R.ms;
+      for (int c = 0; c < A.C; ++c) {
+        A.bias[c] = op.bias_off >= 0 ? host_blob[op.bias_off + c] : 0.f;
+        A.sm1[c] = op.slope_off >= 0 ? host_blob[op.slope_off + c] - 1.f : 0.f;
+        A.proj[c] = A.has_proj ? host_blob[op.ext_off[0] + c] : 0.f;
+      }
+      A.proj_b = A.has_proj && op.ext_off[1] >= 0 ? host_blob[op.ext_off[1]] : 0.f;
+    }
+  }
   // tensor-core MIX ops read their weights as 16-bit [chunk][tap][m16_total][kc + 8] blocks: pack them here, once per
   // weight update, so the kernels stage them with plain 16-byte copies
   std::vector<std::vector<uint16_t>> keep;
   for (size_t i = 0; i < P->ops.size(); ++i) {
-    const TcChoice& tc = P->op_tc[i];
-    if (tc.mt <= 0) continue;
+    const OpLaunch& R = P->launch[i];
+    if (R.kern != Kern::MixTc) continue;
+    const TcChoice& tc = R.tc;
     const csnet_op_desc& op = P->ops[i];
     const int C = mix_channels(*P, op), slice = tc.mt * 16, m16t = (C + slice - 1) / slice * slice, WR = tc.kc + 8;
     for (int p = 0; p < op.n_paths; ++p) {
@@ -930,7 +920,7 @@ int csnet_plan_set_blob(csnet_plan* P, const float* host_blob, int64_t n, void* 
             else { __nv_bfloat16 hv = __float2bfloat16_rn(v); memcpy(&bits, &hv, 2); }
             h[(((size_t)(ci / tc.kc) * kk + tap) * m16t + q.cout0 + co) * WR + ci % tc.kc] = bits;
           }
-      CU_CHECK(cudaMemcpyAsync(P->op_w16[i][p], h.data(), h.size() * 2, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+      CU_CHECK(cudaMemcpyAsync(R.w16[p], h.data(), h.size() * 2, cudaMemcpyHostToDevice, (cudaStream_t)stream));
       keep.push_back(std::move(h));
     }
   }
@@ -950,7 +940,8 @@ static int check_run_args(csnet_plan* P, int32_t N, const void* const* ext_ptrs,
 static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_ptrs, cudaStream_t stream) {
   const csnet_op_desc& op = P->ops[i];
   const csnet_tensor_desc& D = P->tensors[op.dst];
-  switch (P->op_kern[i]) {
+  const OpLaunch& R = P->launch[i];
+  switch (R.kern) {
     case Kern::Msd:
       // MSBlock: one launch per dilated path on the FP32 pipe (ms_direct.cuh)
       for (int p = 0; p < op.n_paths; ++p) {
@@ -967,10 +958,20 @@ static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_
       break;
     case Kern::MixStream: {
       // streaming 1x1 MIX kernel (mix_stream.cuh): TMA operand tiles -> wgmma -> epilogue (resample-adds, PReLU, projection)
-      csnet::MsArgs A;
+      csnet::MsArgs A = R.ms;
+      A.N = N;
+      A.total_chunks = N * A.cpi;
+      A.dst = P->tensor_ptr(op.dst, N, ext_ptrs);
       CUtensorMap maps[csnet::kMsMaxIn];
       memset(maps, 0, sizeof maps);
-      if (!make_ms(*P, op, N, ext_ptrs, &A, maps)) return fail(CSNET_E_UNSUPPORTED, "MIX op no longer qualifies for the streaming kernel");
+      for (int p = 0, in = 0, rs = 0; p < op.n_paths; ++p) {         // numbered as plan_ms does: each kind in path order
+        const csnet_path_desc& q = op.paths[p];
+        const csnet_tensor_desc& S = P->tensors[q.src];
+        if (q.ksize == 0) { A.rsrc[rs++] = P->tensor_ptr(q.src, N, ext_ptrs); continue; }
+        if (!encode_group_map(&maps[in], P->tensor_ptr(q.src, N, ext_ptrs), N, S.C, S.H, S.W, A.S[in], A.G, csnet::kMsRows + (A.k3 ? 2 : 0)))
+          return fail(CSNET_E_CUDA, "cuTensorMapEncodeTiled failed (streaming MIX)");
+        ++in;
+      }
       for (int k = A.n_in; k < csnet::kMsMaxIn; ++k) maps[k] = maps[0];
       int grid = A.total_chunks / 2;
       grid = grid < 1 ? 1 : (grid > P->num_sms ? P->num_sms : grid);
@@ -979,15 +980,15 @@ static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_
     }
     case Kern::MixTc: {
       csnet::MixArgs A = make_mix(*P, op, N, ext_ptrs);
-      const TcChoice& tc = P->op_tc[i];
+      const TcChoice& tc = R.tc;
       const int Cm = A.C;
       csnet::TcGeom G{};
       G.tiles_x = (D.W + csnet::kTcTW - 1) / csnet::kTcTW; G.xs_halves = tc.xs_halves; G.kc = tc.kc; G.rows = tc.rows;
       const int th = csnet::kTcTH * tc.rows;
       G.m16_total = (Cm + tc.mt * 16 - 1) / (tc.mt * 16) * (tc.mt * 16);
-      for (int p = 0; p < op.n_paths; ++p) G.w16[p] = P->op_w16[i][p];
+      for (int p = 0; p < op.n_paths; ++p) G.w16[p] = R.w16[p];
       dim3 grid(G.tiles_x * ((D.H + th - 1) / th), (Cm + tc.mt * 16 - 1) / (tc.mt * 16), N);
-      launch_mix_tc(tc, grid, P->op_smem[i], stream, A, G);
+      R.tc_fn<<<grid, csnet::kTcThreads, R.smem, stream>>>(A, G);
       break;
     }
     case Kern::Pool2: {
@@ -1030,15 +1031,9 @@ static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_
     }
     case Kern::IlStream: {
       // streaming kernel (il_stream.cuh): TMA operand tiles, wgmma GEMM, register-resident depthwise tail
-      csnet::IlsArgs A;
-      if (!make_ils(*P, op, &A)) return fail(CSNET_E_UNSUPPORTED, "ILBLOCK op no longer qualifies for the streaming kernel");
-      auto f = [&](int e) { return op.ext_off[e] >= 0 ? P->blob + op.ext_off[e] : nullptr; };
+      csnet::IlsArgs A = R.ils;
       A.yh = P->tensor_ptr(op.dst, N, ext_ptrs);
       A.yl = op.dst2 >= 0 ? P->tensor_ptr(op.dst2, N, ext_ptrs) : nullptr;
-      A.wh = reinterpret_cast<const uint32_t*>(f(0));
-      A.wl = reinterpret_cast<const uint32_t*>(f(1));
-      A.dw1h = {f(6), f(7), f(8)};   A.dw1l = {f(9), f(10), f(11)};
-      A.dw2h = {f(12), f(13), f(14)}; A.dw2l = {f(15), f(16), f(17)};
       A.N = N;
       A.total_chunks = N * A.ns * A.cpi;
       CUtensorMap tmH, tmL;
@@ -1057,12 +1052,14 @@ static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_
       break;
     }
     case Kern::IlBlock: {
-      csnet::IlArgs A;
-      if (!make_il(*P, op, N, ext_ptrs, &A)) return fail(CSNET_E_UNSUPPORTED, "ILBLOCK op does not fit shared memory");
+      csnet::IlArgs A = R.il;
+      A.xh = P->tensor_ptr(op.paths[0].src, N, ext_ptrs);
+      if (!A.first) A.xl = P->tensor_ptr(op.paths[1].src, N, ext_ptrs);   // (the stem form has no lo input tensor)
+      A.yh = P->tensor_ptr(op.dst, N, ext_ptrs);
+      if (op.dst2 >= 0) A.yl = P->tensor_ptr(op.dst2, N, ext_ptrs);
       const int tiles_y = (A.H + A.TH - 1) / A.TH;
       dim3 grid(A.tiles_x * tiles_y, 1, N);
-      if (D.dtype == CSNET_F16) launch_il_t<__half>(A, grid, P->op_smem[i], stream);
-      else launch_il_t<__nv_bfloat16>(A, grid, P->op_smem[i], stream);
+      R.il_fn<<<grid, csnet::kIlThreads, R.smem, stream>>>(A);
       break;
     }
     case Kern::DwFast:
@@ -1076,7 +1073,7 @@ static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_
       A.bias = op.bias_off >= 0 ? P->blob + op.bias_off : nullptr;
       A.slope = op.slope_off >= 0 ? P->blob + op.slope_off : nullptr;
       A.src_dtype = S.dtype; A.dst_dtype = D.dtype; A.C = D.C; A.H = D.H; A.W = D.W;
-      if (P->op_kern[i] == Kern::DwFast) {
+      if (R.kern == Kern::DwFast) {
         const int tasks = (D.W / 4) * ((D.H + csnet::kDwfRun - 1) / csnet::kDwfRun);
         dim3 grid((tasks + csnet::kDwfThreads - 1) / csnet::kDwfThreads, D.C, N);
         if (D.dtype == CSNET_F16) csnet::dw_fast_kernel<__half><<<grid, csnet::kDwfThreads, 0, stream>>>(A);
@@ -1198,20 +1195,15 @@ int csnet_plan_read_tensor(csnet_plan* P, int32_t tensor, int32_t N, void* dst, 
 
 // Which kernel launch_op() runs for op i, by name (bench.py groups per-op times by kernel).
 const char* csnet_plan_op_kernel(const csnet_plan* P, int32_t i) {
-  static const char* const names[] = {
-      "msd_kernel (ms_direct.cuh, FP32 pipe)", "mix_stream_kernel (TMA + wgmma)", "mix_tc_kernel (mma.sync)",
-      "pool2 / upsample / resample kernels", "pool2 / upsample / resample kernels", "pool2 / upsample / resample kernels",
-      "mix_generic_kernel", "gn kernels", "il_stream_kernel (TMA + wgmma)", "il_block_kernel (mma.sync, tiled)", "dw kernels", "dw kernels"};
-  static_assert(sizeof names / sizeof names[0] == (size_t)Kern::DwGeneric + 1, "one name per Kern");
   if (!P || i < 0 || i >= (int32_t)P->ops.size()) return "";
-  return names[(int)P->op_kern[i]];
+  return kKernNames[(int)P->launch[i].kern];
 }
 
 int32_t csnet_plan_launches(const csnet_plan* P) {
   if (!P) return 0;
   int32_t n = 0;
   for (size_t i = 0; i < P->ops.size(); ++i)
-    n += P->op_kern[i] == Kern::Gn ? 2 : (P->op_kern[i] == Kern::Msd ? P->ops[i].n_paths : 1);
+    n += P->launch[i].kern == Kern::Gn ? 2 : (P->launch[i].kern == Kern::Msd ? P->ops[i].n_paths : 1);
   return n;
 }
 
@@ -1225,8 +1217,8 @@ void csnet_plan_destroy(csnet_plan* P) {
   if (P->blob) cudaFree(P->blob);
   if (P->arena) cudaFree(P->arena);
   if (P->gn_stats) cudaFree(P->gn_stats);
-  for (auto& v : P->op_w16)
-    for (uint16_t* q : v)
+  for (const OpLaunch& R : P->launch)
+    for (uint16_t* q : R.w16)
       if (q) cudaFree(q);
   for (int b = 0; b < 2; ++b) {
     if (P->h_in[b]) cudaFree(P->h_in[b]);

@@ -245,6 +245,25 @@ def test_fused_ilblock_kernel_matches_generic_ops(tag, hw, dtype):
     assert (y - ref).abs().max().item() <= (SIG_TOL_FP16 if dtype == "fp16" else SIG_TOL_BF16)
 
 
+def test_creating_a_plan_leaves_existing_plans_runnable():
+    """A kernel's dynamic shared-memory limit is a property of the kernel, not of a plan, so creating a plan must not change
+    what an existing plan can launch.  At 224x224 the fp16 csnet-L-x2 program runs stage3.1 on the tiled ILBlock kernel
+    with 224 848 bytes of shared memory (W = 56 keeps it off the streaming kernel); the 96x160 program's tiled ILBlock ops
+    need at most 211 936 bytes.  Batch 16 launches op by op; batch 2 replays a captured graph."""
+    cfg, sd = fixtures.checkpoint("csnet-L-x2")
+    a = runtime.Plan(compiler.compile_csnet(cfg, sd, 224, 224, "fp16"), max_batch=16)
+    stage31 = next(i for i, o in enumerate(a.prog.ops) if o.name == "stage3.1")
+    assert a.op_kernel(stage31) == "il_block_kernel (mma.sync, tiled)"
+    x = torch.from_numpy(synth.randn_images(16, 224, 224, 21)).cuda()
+    y16, y2 = a.forward(x), a.forward(x[:2])
+    b = runtime.Plan(compiler.compile_csnet(cfg, sd, 96, 160, "fp16"), max_batch=4)
+    assert torch.isfinite(b.forward(torch.from_numpy(synth.randn_images(4, 96, 160, 22)).cuda())).all()
+    assert torch.equal(a.forward(x), y16)
+    assert torch.equal(a.forward(x[:2]), y2)
+    a.close()
+    b.close()
+
+
 @pytest.mark.parametrize("tag,hw,dtype", [("csnet-L-x2", (224, 224), "fp16"), ("csnet-L-x2", (96, 160), "fp16"),
                                           ("csnet-L-x1", (64, 64), "bf16"), ("init-3br", (128, 128), "fp16")])
 def test_tensor_core_mix_kernel_matches_generic_ops(tag, hw, dtype):
