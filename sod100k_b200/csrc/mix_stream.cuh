@@ -4,13 +4,15 @@
 //
 //   dst[c] = PReLU( bias[c] + sum_i W_i . x_i  +  sum_r bilinear_up(low_r)[c] )          (then, MIXPROJ: dot with proj_w)
 //
-//   * every conv path is a plain 1x1 over a 16-bit tensor at the destination's resolution (W % 8 == 0).  A 2-row chunk of
-//     each input arrives by cp.async.bulk.tensor.5d in the tensor-core operand layout [row][8-px group][slot][8 px]
-//     (channel slots past C zero-filled = the K padding): the threads never touch the operands.
+//   * every conv path is a plain 1x1 over a 16-bit tensor at the destination's resolution (W % 8 == 0).  A chunk of A.rows
+//     rows (chosen per op by the plan) of each input arrives by cp.async.bulk.tensor.5d in the tensor-core operand layout
+//     [row][8-px group][slot][8 px] (channel slots past C zero-filled = the K padding): the threads never touch the operands.
+//     Under the same barrier, cp.async.bulk.tensor.4d brings the fp32 rows of each resample-add source that the chunk's
+//     bilinear taps reach.
 //   * warp 0 (one lane) is the TMA producer over a ring of stages; kMsGroups consumer warpgroups share the 64-pixel blocks
 //     of each chunk: wgmma.mma_async (M = 64 pixels, N = ru16(Cout), K = 16 per instruction, the paths of the op accumulate
 //     into the same registers = K-concatenation), then the epilogue from the accumulator fragment: bias, the op's
-//     resample-add paths (fp32 low-resolution conv results of the up-paths, gathered bilinearly from L2), PReLU, then
+//     resample-add paths (fp32 low-resolution conv results of the up-paths, gathered bilinearly from shared memory), PReLU, then
 //     either stores of the Cout planes or the projection onto one fp32 channel (cls_layer) — the Cout-channel tensor is
 //     never written.  While one warpgroup runs its epilogue, the others' MMAs and the producer's loads are in flight.
 // 3x3 form (k3: every conv path a 3x3, pad 1 — the stage-entry gOctaveCBR of stride-2 ILBlocks, csnet.py:60-71 with the
@@ -23,19 +25,19 @@
 
 namespace csnet {
 
-constexpr int kMsMaxIn = 3, kMsMaxRs = 2, kMsMaxC = 80, kMsRows = 2;
+constexpr int kMsMaxIn = 3, kMsMaxRs = 2, kMsMaxC = 80, kMsRows = 2;   // kMsRows: the chunk height the kernel choice is judged by
 constexpr int kMsGroups = 3, kMsThreads = (4 + 4 * kMsGroups) * 32;   // warp 0: TMA; 2, 3: 3x3 builders; 4..: consumer warpgroups
 
 struct MsArgs {
   void* dst;
   const float* w[kMsMaxIn];             // fp32 [cin][cout] of each conv path
-  const void* rsrc[kMsMaxRs];           // resample-add sources [N][rC][rH][rW]
   float bias[kMsMaxC], sm1[kMsMaxC], proj[kMsMaxC];
   float proj_b;
   int32_t has_proj, has_slope, dst_f32;
   int32_t n_in, cin[kMsMaxIn], cout0[kMsMaxIn], cout[kMsMaxIn], S[kMsMaxIn], K16[kMsMaxIn], in_off[kMsMaxIn];
   int32_t n_rs, r_dtype[kMsMaxRs], r_up[kMsMaxRs], r_H[kMsMaxRs], r_W[kMsMaxRs], r_C[kMsMaxRs], r_c0[kMsMaxRs], r_cout0[kMsMaxRs], r_n[kMsMaxRs];
-  int32_t N, H, W, C, NN, G, nb;        // destination dims; NN = ru16(C); G = W / 8; nb = 64-pixel GEMM blocks per chunk
+  int32_t r_rows[kMsMaxRs], r_off[kMsMaxRs];   // low-resolution rows a chunk's taps reach; their tile's offset in a stage
+  int32_t N, H, W, C, NN, G, nb, rows;  // destination dims; NN = ru16(C); G = W / 8; nb = 64-pixel GEMM blocks per chunk of `rows` rows
   int32_t k3, copy_bytes[kMsMaxIn];     // 3x3 form; bytes of one of the three copies (centre, x-1, x+1) of input i's tile
   int32_t cpi, total_chunks, n_stages, stage_bytes, tx_bytes;
   int32_t off_stage, off_wb[kMsMaxIn], off_bar, off_tab, smem_bytes;
@@ -45,7 +47,7 @@ struct MsTap {                           // bilinear taps of one destination pix
   int32_t o00, o01, o10, o11;
   float w00, w01, w10, w11;
 };
-__device__ __forceinline__ MsTap ms_tap(int Hs, int Ws, int up, int oy, int ox) {
+__host__ __device__ __forceinline__ MsTap ms_tap(int Hs, int Ws, int up, int oy, int ox) {
   // F.interpolate(bilinear, align_corners=False): source index (dst + 0.5) / up - 0.5, clamped at 0; the +1 neighbour clamped
   const float inv = 1.0f / (float)up;
   float sy = ((float)oy + 0.5f) * inv - 0.5f, sx = ((float)ox + 0.5f) * inv - 0.5f;
@@ -59,6 +61,9 @@ __device__ __forceinline__ MsTap ms_tap(int Hs, int Ws, int up, int oy, int ox) 
   t.w00 = hy * hx; t.w01 = hy * lx; t.w10 = ly * hx; t.w11 = ly * lx;
   return t;
 }
+__device__ __forceinline__ float ldsf(uint32_t a) { return __uint_as_float(lds32(a)); }
+// The first low-resolution row that the taps of destination row oy reach: the top row of a chunk's staged source tile.
+__host__ __device__ __forceinline__ int ms_row0(int Hs, int Ws, int up, int oy) { return ms_tap(Hs, Ws, up, oy, 0).o00 / Ws; }
 
 // Consumer warpgroup `wg`: the (chunk, block) tasks t = k * nb + blk with t % kMsGroups == wg.  A task = one 64-pixel
 // block: wgmma over every conv path (and tap) of the op into one fp32 accumulator fragment, then the epilogue from the
@@ -68,8 +73,8 @@ __device__ __forceinline__ MsTap ms_tap(int Hs, int Ws, int up, int oy, int ox) 
 // Every warpgroup waits for every chunk and releases its stage once (bar_empty counts kMsGroups arrivals), so the
 // barriers' phases never run ahead of a warpgroup that has no task in a chunk.
 template <typename T, int NRS, bool PROJ, int NN>
-__device__ __forceinline__ void ms_consume(const MsArgs& A, uint32_t sbase, uint32_t STG, uint32_t tab, uint32_t bar_ready, uint32_t bar_empty,
-                                           int ra, int rb, int wg, int qd, int lane) {
+__device__ __forceinline__ void ms_consume(const MsArgs& A, uint32_t sbase, uint32_t STG, uint32_t tab, uint32_t bar_full, uint32_t bar_ready,
+                                           uint32_t bar_empty, int ra, int rb, int wg, int qd, int lane) {
   const int H = A.H, W = A.W, C = A.C, G = A.G, nb = A.nb, NS = A.n_stages, taps = A.k3 ? 9 : 1;
   const size_t plane = (size_t)H * W;
   const int q = lane & 3;
@@ -77,6 +82,14 @@ __device__ __forceinline__ void ms_consume(const MsArgs& A, uint32_t sbase, uint
     const int s = k % NS, n = idx / A.cpi, c = idx - n * A.cpi;
     const uint32_t st = STG + (uint32_t)s * (uint32_t)A.stage_bytes;
     mbar_wait_a(bar_ready + 8 * s, (uint32_t)(k / NS) & 1u);
+    if (NRS > 0 && A.k3) mbar_wait_a(bar_full + 8 * s, (uint32_t)(k / NS) & 1u);   // the source tiles, read by these threads
+    // staged source tile j: [r_n channels][r_rows rows from ms_row0][r_W]; rsb[j] addresses its (virtual) row 0
+    uint32_t rsb[NRS > 0 ? NRS : 1], rcs[NRS > 0 ? NRS : 1];
+#pragma unroll
+    for (int j = 0; j < NRS; ++j) {
+      rcs[j] = (uint32_t)(A.r_rows[j] * A.r_W[j]) * 4u;
+      rsb[j] = st + (uint32_t)A.r_off[j] - (uint32_t)(ms_row0(A.r_H[j], A.r_W[j], A.r_up[j], c * A.rows) * A.r_W[j]) * 4u;
+    }
     for (int blk = 0; blk < nb; ++blk) {
       if ((k * nb + blk) % kMsGroups != wg) continue;                      // warpgroup-uniform
       float d[NN / 2];
@@ -102,18 +115,12 @@ __device__ __forceinline__ void ms_consume(const MsArgs& A, uint32_t sbase, uint
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int p = blk * 64 + qd * 16 + (lane >> 2) + 8 * h, pg = p >> 3;
-        const bool valid = pg < kMsRows * G;
+        const bool valid = pg < A.rows * G;
         const int r = pg / G, g = pg - r * G;
-        const int y = valid ? c * kMsRows + r : 0, x = valid ? 8 * g + (p & 7) : 0;
+        const int y = valid ? c * A.rows + r : c * A.rows, x = valid ? 8 * g + (p & 7) : 0;   // (invalid: a row of the tile)
         MsTap tp[NRS > 0 ? NRS : 1];
-        const float* rs[NRS > 0 ? NRS : 1];
-        int rpl[NRS > 0 ? NRS : 1];
 #pragma unroll
-        for (int j = 0; j < NRS; ++j) {
-          tp[j] = ms_tap(A.r_H[j], A.r_W[j], A.r_up[j], y, x);
-          rpl[j] = A.r_H[j] * A.r_W[j];
-          rs[j] = reinterpret_cast<const float*>(A.rsrc[j]) + ((size_t)n * A.r_C[j] + (size_t)A.r_c0[j]) * (size_t)rpl[j];
-        }
+        for (int j = 0; j < NRS; ++j) tp[j] = ms_tap(A.r_H[j], A.r_W[j], A.r_up[j], y, x);
         float proj_acc = 0.f;
 #pragma unroll
         for (int i = 0; i < NN / 8; ++i) {
@@ -125,9 +132,9 @@ __device__ __forceinline__ void ms_consume(const MsArgs& A, uint32_t sbase, uint
 #pragma unroll
             for (int t = 0; t < NRS; ++t) {
               if (ch < A.r_n[t]) {                                            // (resample-add paths cover channels [0, r_n): checked by the host)
-                const float* s_ = rs[t] + ch * rpl[t];
-                v += tp[t].w00 * __ldg(s_ + tp[t].o00) + tp[t].w01 * __ldg(s_ + tp[t].o01) + tp[t].w10 * __ldg(s_ + tp[t].o10) +
-                     tp[t].w11 * __ldg(s_ + tp[t].o11);
+                const uint32_t s_ = rsb[t] + (uint32_t)ch * rcs[t];
+                v += tp[t].w00 * ldsf(s_ + 4u * (uint32_t)tp[t].o00) + tp[t].w01 * ldsf(s_ + 4u * (uint32_t)tp[t].o01) +
+                     tp[t].w10 * ldsf(s_ + 4u * (uint32_t)tp[t].o10) + tp[t].w11 * ldsf(s_ + 4u * (uint32_t)tp[t].o11);
               }
             }
             v = prelu_m1(v, __uint_as_float(t4.y));
@@ -152,21 +159,21 @@ __device__ __forceinline__ void ms_consume(const MsArgs& A, uint32_t sbase, uint
 }
 
 template <typename T, int NRS, bool PROJ>
-__device__ __forceinline__ void ms_consume_n(const MsArgs& A, uint32_t sbase, uint32_t STG, uint32_t tab, uint32_t bar_ready, uint32_t bar_empty,
-                                             int ra, int rb, int wg, int qd, int lane) {
+__device__ __forceinline__ void ms_consume_n(const MsArgs& A, uint32_t sbase, uint32_t STG, uint32_t tab, uint32_t bar_full, uint32_t bar_ready,
+                                             uint32_t bar_empty, int ra, int rb, int wg, int qd, int lane) {
   switch (A.NN) {
-    case 16: ms_consume<T, NRS, PROJ, 16>(A, sbase, STG, tab, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
-    case 32: ms_consume<T, NRS, PROJ, 32>(A, sbase, STG, tab, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
-    case 48: ms_consume<T, NRS, PROJ, 48>(A, sbase, STG, tab, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
-    case 64: ms_consume<T, NRS, PROJ, 64>(A, sbase, STG, tab, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
-    default: ms_consume<T, NRS, PROJ, 80>(A, sbase, STG, tab, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
+    case 16: ms_consume<T, NRS, PROJ, 16>(A, sbase, STG, tab, bar_full, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
+    case 32: ms_consume<T, NRS, PROJ, 32>(A, sbase, STG, tab, bar_full, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
+    case 48: ms_consume<T, NRS, PROJ, 48>(A, sbase, STG, tab, bar_full, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
+    case 64: ms_consume<T, NRS, PROJ, 64>(A, sbase, STG, tab, bar_full, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
+    default: ms_consume<T, NRS, PROJ, 80>(A, sbase, STG, tab, bar_full, bar_ready, bar_empty, ra, rb, wg, qd, lane); break;
   }
 }
 
 template <typename T>
 __global__ void __launch_bounds__(kMsThreads, 1)
 mix_stream_kernel(const __grid_constant__ MsArgs A, const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
-                  const __grid_constant__ CUtensorMap tm2) {
+                  const __grid_constant__ CUtensorMap tm2, const __grid_constant__ CUtensorMap tr0, const __grid_constant__ CUtensorMap tr1) {
   extern __shared__ uint8_t smem_raw[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t sbase = (smem_u32(smem_raw) + 127u) & ~127u;
@@ -198,7 +205,7 @@ mix_stream_kernel(const __grid_constant__ MsArgs A, const __grid_constant__ CUte
     }
     if (A.k3) {
       // K-padding slots [cin, S) of the two shifted copies of every stage: zero once (the builders only write real channels)
-      const int tg = (kMsRows + 2) * A.G, per = A.S[i] - A.cin[i];
+      const int tg = (A.rows + 2) * A.G, per = A.S[i] - A.cin[i];
       for (int e = tid; e < NS * 2 * tg * per; e += kMsThreads) {
         const int st = e / (2 * tg * per), r2 = e - st * 2 * tg * per, cp = r2 / (tg * per), r3 = r2 - cp * tg * per, g_ = r3 / per, k_ = A.cin[i] + (r3 - g_ * per);
         sts128(STG + (uint32_t)st * (uint32_t)A.stage_bytes + (uint32_t)A.in_off[i] + (uint32_t)(cp + 1) * (uint32_t)A.copy_bytes[i] + (uint32_t)(g_ * A.S[i] + k_) * 16u,
@@ -220,17 +227,20 @@ mix_stream_kernel(const __grid_constant__ MsArgs A, const __grid_constant__ CUte
         if (k >= NS) mbar_wait_a(bar_empty + 8 * s, ((uint32_t)(k / NS) - 1u) & 1u);      // every consumer is done with the stage
         const uint32_t bar = bar_full + 8 * s, st = STG + (uint32_t)s * (uint32_t)A.stage_bytes;
         mbar_expect_tx_a(bar, (uint32_t)A.tx_bytes);
-        const int y0 = kMsRows * c - (A.k3 ? 1 : 0);                       // 3x3: one halo row above (and below: the box is 2 rows taller)
+        const int y0 = A.rows * c - (A.k3 ? 1 : 0);                        // 3x3: one halo row above (and below: the box is 2 rows taller)
         tma_load_5d(st + (uint32_t)A.in_off[0], &tm0, bar, 0, 0, 0, y0, n);
         if (A.n_in > 1) tma_load_5d(st + (uint32_t)A.in_off[1], &tm1, bar, 0, 0, 0, y0, n);
         if (A.n_in > 2) tma_load_5d(st + (uint32_t)A.in_off[2], &tm2, bar, 0, 0, 0, y0, n);
+        // resample-add sources: the low-resolution rows this chunk's bilinear taps reach (rows past the bottom: zero fill, never read)
+        if (A.n_rs > 0) tma_load_4d_a(st + (uint32_t)A.r_off[0], &tr0, bar, 0, ms_row0(A.r_H[0], A.r_W[0], A.r_up[0], A.rows * c), A.r_c0[0], n);
+        if (A.n_rs > 1) tma_load_4d_a(st + (uint32_t)A.r_off[1], &tr1, bar, 0, ms_row0(A.r_H[1], A.r_W[1], A.r_up[1], A.rows * c), A.r_c0[1], n);
       }
     }
   } else if (warp == 2 || warp == 3) {
     // ---- 3x3 form: builders of the shifted copies.  Copy 1 holds x-1 (pixel j of a group = pixel j-1 of the centre tile),
     //      copy 2 holds x+1; zeros enter at the image's left / right edge ---------------------------------------------------
     if (A.k3) {
-      const int bt = (warp - 2) * 32 + lane, G = A.G, tg = (kMsRows + 2) * G;
+      const int bt = (warp - 2) * 32 + lane, G = A.G, tg = (A.rows + 2) * G;
       for (int idx = ra, k = 0; idx < rb; ++idx, ++k) {
         const int s = k % NS;
         mbar_wait_a(bar_full + 8 * s, (uint32_t)(k / NS) & 1u);
@@ -256,10 +266,10 @@ mix_stream_kernel(const __grid_constant__ MsArgs A, const __grid_constant__ CUte
   } else if (warp >= 4) {
     const int e = warp - 4, qd = e & 3, wg = e >> 2;
     const uint32_t ready = A.k3 ? bar_built : bar_full;
-    if (A.has_proj) ms_consume_n<T, 0, true>(A, sbase, STG, TAB, ready, bar_empty, ra, rb, wg, qd, lane);
-    else if (A.n_rs == 0) ms_consume_n<T, 0, false>(A, sbase, STG, TAB, ready, bar_empty, ra, rb, wg, qd, lane);
-    else if (A.n_rs == 1) ms_consume_n<T, 1, false>(A, sbase, STG, TAB, ready, bar_empty, ra, rb, wg, qd, lane);
-    else ms_consume_n<T, 2, false>(A, sbase, STG, TAB, ready, bar_empty, ra, rb, wg, qd, lane);
+    if (A.has_proj) ms_consume_n<T, 0, true>(A, sbase, STG, TAB, bar_full, ready, bar_empty, ra, rb, wg, qd, lane);
+    else if (A.n_rs == 0) ms_consume_n<T, 0, false>(A, sbase, STG, TAB, bar_full, ready, bar_empty, ra, rb, wg, qd, lane);
+    else if (A.n_rs == 1) ms_consume_n<T, 1, false>(A, sbase, STG, TAB, bar_full, ready, bar_empty, ra, rb, wg, qd, lane);
+    else ms_consume_n<T, 2, false>(A, sbase, STG, TAB, bar_full, ready, bar_empty, ra, rb, wg, qd, lane);
   }
 }
 

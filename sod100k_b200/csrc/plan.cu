@@ -479,13 +479,14 @@ bool encode_group_map(CUtensorMap* tm, const void* base, int N, int C, int H, in
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// 4-D map over the planar fp32 image [N][C][H][W]: box (bw floats, rows, C, 1) -> [c][row][bw] in shared memory, zeros outside.
-bool encode_image_map(CUtensorMap* tm, const void* base, int N, int C, int H, int W, int bw, int rows) {
+// 4-D map over a planar fp32 tensor [N][C][H][W]: box (bw floats, rows, bc channels, 1) -> [c][row][bw] in shared memory,
+// zeros outside.
+bool encode_image_map(CUtensorMap* tm, const void* base, int N, int C, int H, int W, int bw, int rows, int bc) {
   EncodeTiledFn fn = encode_tiled_fn();
   if (!fn) return false;
   const cuuint64_t dims[4] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)C, (cuuint64_t)N};
   const cuuint64_t strides[3] = {(cuuint64_t)W * 4, (cuuint64_t)H * W * 4, (cuuint64_t)C * H * W * 4};
-  const cuuint32_t box[4] = {(cuuint32_t)bw, (cuuint32_t)rows, (cuuint32_t)C, 1};
+  const cuuint32_t box[4] = {(cuuint32_t)bw, (cuuint32_t)rows, (cuuint32_t)bc, 1};
   const cuuint32_t estr[4] = {1, 1, 1, 1};
   return fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<void*>(base), dims, strides, box, estr,
             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
@@ -599,6 +600,7 @@ bool plan_ms(const csnet_plan& P, const csnet_op_desc& op, csnet::MsArgs* out) {
     const csnet_tensor_desc& S = P.tensors[q.src];
     if (q.ksize == 0) {
       if (A.n_rs >= csnet::kMsMaxRs || q.up < 2 || q.pool != 1 || q.pre_avg || S.H * q.up != D.H || S.W * q.up != D.W || S.dtype != CSNET_F32 || q.cout0 != 0) return false;
+      if (S.W % 4 || S.W > 256 || q.cout > 256) return false;                 // a TMA box row: a multiple of 16 bytes, <= 256 elements
       const int j = A.n_rs++;
       A.r_dtype[j] = S.dtype; A.r_up[j] = q.up; A.r_H[j] = S.H; A.r_W[j] = S.W; A.r_C[j] = S.C; A.r_c0[j] = q.c0; A.r_cout0[j] = q.cout0; A.r_n[j] = q.cout;
       continue;
@@ -608,35 +610,69 @@ bool plan_ms(const csnet_plan& P, const csnet_op_desc& op, csnet::MsArgs* out) {
         S.dtype != CSNET_F16 || S.H != D.H || S.W != D.W || q.cin > 64)
       return false;
     A.k3 = k3;
-    const int trows = csnet::kMsRows + (k3 ? 2 : 0);
     const int i = A.n_in++;
     A.w[i] = P.blob + q.w_off;
     A.cin[i] = q.cin; A.cout0[i] = q.cout0; A.cout[i] = q.cout;
     A.K16[i] = round_up(q.cin, 16); A.S[i] = A.K16[i] + 1;
-    A.in_off[i] = off;
-    A.copy_bytes[i] = r128(trows * A.G * A.S[i] * 16);
-    off += (k3 ? 3 : 1) * A.copy_bytes[i];
     if (q.c0 != 0) return false;                                           // (a channel-sliced source would need a c0 coordinate)
   }
   if (A.n_in == 0) return false;
-  A.stage_bytes = off;
-  A.tx_bytes = 0;
-  for (int i = 0; i < A.n_in; ++i) A.tx_bytes += (csnet::kMsRows + (A.k3 ? 2 : 0)) * A.G * A.S[i] * 16;
-  A.nb = (csnet::kMsRows * A.G + 7) / 8;
-  A.cpi = D.H / csnet::kMsRows;
-  int wb = 0;
   const int taps = A.k3 ? 9 : 1;
-  for (int i = 0; i < A.n_in; ++i) wb += r128(taps * A.NN * A.K16[i] * 2);
-  const int fixed = wb + 512 + 1280 + 16 * 65 * 16 + 128;                  // weights, barriers, tables, tail slack, alignment
-  A.n_stages = (227 * 1024 - fixed) / A.stage_bytes;
-  A.n_stages = A.n_stages > 6 ? 6 : A.n_stages;
-  if (A.n_stages < 2) return false;
-  A.off_stage = 0;
-  int o = A.n_stages * A.stage_bytes + 16 * 65 * 16;
-  for (int i = 0; i < A.n_in; ++i) { A.off_wb[i] = o; o += r128(taps * A.NN * A.K16[i] * 2); }
-  A.off_bar = o; o += 512;
-  A.off_tab = o; o += 1280;
-  A.smem_bytes = o + 128;
+  int wb = 0, smax = 0;
+  for (int i = 0; i < A.n_in; ++i) { wb += r128(taps * A.NN * A.K16[i] * 2); smax = A.S[i] > smax ? A.S[i] : smax; }
+  // the stage layout of a chunk height: per input its tile (3x3: and the two shifted copies), then per resample path the
+  // fp32 box [r_n][r_rows][r_W] of the low-resolution rows that a chunk's taps reach
+  auto shape = [&](int rows) {
+    csnet::MsArgs T = A;
+    T.rows = rows;
+    T.nb = (rows * T.G + 7) / 8;
+    T.cpi = D.H / rows;
+    int off = 0;
+    T.tx_bytes = 0;
+    for (int i = 0; i < T.n_in; ++i) {
+      const int trows = rows + (T.k3 ? 2 : 0);
+      T.in_off[i] = off;
+      T.copy_bytes[i] = r128(trows * T.G * T.S[i] * 16);
+      off += (T.k3 ? 3 : 1) * T.copy_bytes[i];
+      T.tx_bytes += trows * T.G * T.S[i] * 16;
+    }
+    for (int j = 0; j < T.n_rs; ++j) {
+      T.r_rows[j] = 0;
+      for (int c = 0; c < T.cpi; ++c) {
+        const int last = csnet::ms_tap(T.r_H[j], T.r_W[j], T.r_up[j], c * rows + rows - 1, 0).o10 / T.r_W[j];
+        const int n = last - csnet::ms_row0(T.r_H[j], T.r_W[j], T.r_up[j], c * rows) + 1;
+        T.r_rows[j] = n > T.r_rows[j] ? n : T.r_rows[j];
+      }
+      T.r_off[j] = off;
+      off += r128(T.r_n[j] * T.r_rows[j] * T.r_W[j] * 4);
+      T.tx_bytes += T.r_n[j] * T.r_rows[j] * T.r_W[j] * 4;
+    }
+    T.stage_bytes = off;
+    // the last block of a chunk reads past the chunk's groups (rows it does not store): slack after the ring keeps that in bounds
+    const int slack = (T.nb * 8 - rows * T.G) * smax * 16;
+    T.n_stages = (227 * 1024 - (wb + slack + 512 + 1280 + 128)) / T.stage_bytes;   // weights, slack, barriers, tables, alignment
+    T.n_stages = T.n_stages > 6 ? 6 : T.n_stages;
+    T.off_stage = 0;
+    int o = T.n_stages * T.stage_bytes + slack;
+    for (int i = 0; i < T.n_in; ++i) { T.off_wb[i] = o; o += r128(taps * T.NN * T.K16[i] * 2); }
+    T.off_bar = o; o += 512;
+    T.off_tab = o; o += 1280;
+    T.smem_bytes = o + 128;
+    return T;
+  };
+  // chunk height: the smallest that divides H, gives every consumer warpgroup a 64-pixel block per chunk and leaves 3 ring
+  // stages; otherwise kMsRows, or 1 row when kMsRows leaves fewer than 2 stages
+  bool found = false;
+  for (int rows = 1; rows <= 16 && !found; ++rows) {
+    if (D.H % rows) continue;
+    const csnet::MsArgs T = shape(rows);
+    if (T.nb >= csnet::kMsGroups && T.n_stages >= 3) { A = T; found = true; }
+  }
+  if (!found) {
+    A = shape(csnet::kMsRows);
+    if (A.n_stages < 2) A = shape(1);
+    if (A.n_stages < 2) return false;
+  }
   A.has_slope = op.slope_off >= 0;
   *out = A;
   return true;
@@ -962,20 +998,26 @@ static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_
       A.N = N;
       A.total_chunks = N * A.cpi;
       A.dst = P->tensor_ptr(op.dst, N, ext_ptrs);
-      CUtensorMap maps[csnet::kMsMaxIn];
+      CUtensorMap maps[csnet::kMsMaxIn], rmaps[csnet::kMsMaxRs];
       memset(maps, 0, sizeof maps);
       for (int p = 0, in = 0, rs = 0; p < op.n_paths; ++p) {         // numbered as plan_ms does: each kind in path order
         const csnet_path_desc& q = op.paths[p];
         const csnet_tensor_desc& S = P->tensors[q.src];
-        if (q.ksize == 0) { A.rsrc[rs++] = P->tensor_ptr(q.src, N, ext_ptrs); continue; }
-        if (!encode_group_map(&maps[in], P->tensor_ptr(q.src, N, ext_ptrs), N, S.C, S.H, S.W, A.S[in], A.G, csnet::kMsRows + (A.k3 ? 2 : 0)))
+        if (q.ksize == 0) {
+          if (!encode_image_map(&rmaps[rs], P->tensor_ptr(q.src, N, ext_ptrs), N, S.C, S.H, S.W, S.W, A.r_rows[rs], A.r_n[rs]))
+            return fail(CSNET_E_CUDA, "cuTensorMapEncodeTiled failed (streaming MIX)");
+          ++rs;
+          continue;
+        }
+        if (!encode_group_map(&maps[in], P->tensor_ptr(q.src, N, ext_ptrs), N, S.C, S.H, S.W, A.S[in], A.G, A.rows + (A.k3 ? 2 : 0)))
           return fail(CSNET_E_CUDA, "cuTensorMapEncodeTiled failed (streaming MIX)");
         ++in;
       }
       for (int k = A.n_in; k < csnet::kMsMaxIn; ++k) maps[k] = maps[0];
+      for (int k = A.n_rs; k < csnet::kMsMaxRs; ++k) rmaps[k] = maps[0];
       int grid = A.total_chunks / 2;
       grid = grid < 1 ? 1 : (grid > P->num_sms ? P->num_sms : grid);
-      csnet::mix_stream_kernel<__half><<<grid, csnet::kMsThreads, A.smem_bytes, stream>>>(A, maps[0], maps[1], maps[2]);
+      csnet::mix_stream_kernel<__half><<<grid, csnet::kMsThreads, A.smem_bytes, stream>>>(A, maps[0], maps[1], maps[2], rmaps[0], rmaps[1]);
       break;
     }
     case Kern::MixTc: {
@@ -1039,7 +1081,7 @@ static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_
       CUtensorMap tmH, tmL;
       const bool stem = A.Ci > 0;
       if (stem) {
-        if (!encode_image_map(&tmL, P->tensor_ptr(op.paths[0].src, N, ext_ptrs), N, A.Ci, A.H, A.W, A.BW, 4))
+        if (!encode_image_map(&tmL, P->tensor_ptr(op.paths[0].src, N, ext_ptrs), N, A.Ci, A.H, A.W, A.BW, 4, A.Ci))
           return fail(CSNET_E_CUDA, "cuTensorMapEncodeTiled failed (streaming ILBlock, image)");
         tmH = tmL;
       } else if (!encode_group_map(&tmH, P->tensor_ptr(op.paths[0].src, N, ext_ptrs), N, A.Chi, A.H, A.W, A.SH, A.GR, 4) ||
