@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define CSNET_ABI_VERSION 5
+#define CSNET_ABI_VERSION 6
 
 enum { CSNET_F32 = 0, CSNET_F16 = 1, CSNET_BF16 = 2 };
 
@@ -190,7 +190,7 @@ void csnet_plan_destroy(csnet_plan* plan);
  * bench.py and of CSNet/test.py:86-93): copies x (fp32 NCHW, N*3*H*W floats) to the device, runs,
  * copies the logits (N*H*W floats) back and returns when y_host is complete.  Batches of 64 or more are cut into
  * three chunks (N/8, the rest, N/8) that pipeline H2D copy / kernels / D2H copy on separate streams (use pinned host memory).
- * Smaller batches, and every batch of csnet_plan_run_host_u8, run as one chunk.
+ * Smaller batches, and every batch of csnet_plan_run_host_u8, run as one chunk (csnet_plan_run_host_images_u8 cuts like this call).
  * The plan must bind external 0 = input, external 1 = logits.
  */
 int csnet_plan_run_host(csnet_plan* plan, int32_t N, const float* x_host, float* y_host, void* stream);
@@ -203,6 +203,41 @@ int csnet_plan_run_host(csnet_plan* plan, int32_t N, const float* x_host, float*
  */
 int csnet_plan_run_host_u8(csnet_plan* plan, int32_t N, const uint8_t* x_hwc, uint8_t* y_u8, const float* mean, const float* std,
                            void* stream);
+
+/*
+ * Images of any size (CSNet/test.py:71-98 with both of its skimage resizes, SURVEY §8 f3).  A ragged batch is packed: image i is
+ * uint8 [h][w][3] at byte src_off of the input, and its saliency map is uint8 [h][w] at byte dst_off of the output.
+ *   in:  resize(img_as_float(img), (H, W), mode='reflect', anti_aliasing=False), then (v - mean[c]) / std[c], all in float64,
+ *        rounded once to the fp32 NCHW network input [N,3,H,W];
+ *   out: sigmoid(logit) in fp32, resize back to (h, w) the same way (float64, rounded to fp32), * 255 truncated to uint8.
+ * The resize is skimage >= 0.19's: scipy.ndimage.zoom(order=1, mode='mirror', grid_mode=True).  At h, w == H, W both sides give
+ * exactly the bytes of csnet_plan_run_host_u8.
+ */
+typedef struct {
+  int64_t src_off;        /* byte offset of the image in the packed input */
+  int64_t dst_off;        /* byte offset of its map in the packed output */
+  int32_t h, w;
+} csnet_image_geom;       /* 24 bytes */
+
+/* Device to device, asynchronous on `stream` (current device): x_packed / geom (DEVICE, N entries) -> x_nchw fp32 [N,3,H,W].
+ * mean / std are host float[3].  The caller guarantees that every image lies inside x_packed (geometry on the device is not checked). */
+int csnet_resize_u8_to_input(const uint8_t* x_packed, const csnet_image_geom* geom, int32_t N, int32_t H, int32_t W, const float* mean,
+                             const float* std, float* x_nchw, void* stream);
+
+/* Device to device, asynchronous on `stream`: logits fp32 [N,1,H,W] -> each image's map at y_packed + dst_off (geometry on the
+ * DEVICE; the maps must not overlap). */
+int csnet_resize_logits_to_u8(const float* logits, int32_t N, int32_t H, int32_t W, const csnet_image_geom* geom, uint8_t* y_packed,
+                              void* stream);
+
+/*
+ * Host to host, synchronised like csnet_plan_run_host: x_packed (x_bytes bytes) and the HOST geometry geom[N] in, the maps out to
+ * y_packed (y_bytes bytes), through the plan's network size H x W.  Every entry is checked before any copy or launch: 1 <= h, w <=
+ * 32767, every image inside x_bytes, every map inside y_bytes, and the maps back to back in input order (each map's dst_off is
+ * where the previous one ends).  Anything else returns CSNET_E_INVALID.  Same pipeline as csnet_plan_run_host (pinned memory for
+ * overlap); the plan's input must have 3 channels.
+ */
+int csnet_plan_run_host_images_u8(csnet_plan* plan, int32_t N, const uint8_t* x_packed, int64_t x_bytes, const csnet_image_geom* geom,
+                                  uint8_t* y_packed, int64_t y_bytes, const float* mean, const float* std, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Training primitives (fp32 planar NCHW device tensors).  The reference trains through torch autograd

@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <cstdint>
 #include <new>
 #include <string>
 #include <vector>
@@ -20,6 +21,7 @@
 #include "ms_direct.cuh"
 #include "mix_tc.cuh"
 #include "dw_fast.cuh"
+#include "image_io.cuh"
 
 namespace {
 
@@ -221,9 +223,11 @@ struct csnet_plan {
   int ils_min_chunks = 592;                       // batches with fewer 4-row chunks per ILBlock run the tiled kernel
   // host-buffer pipeline (csnet_plan_run_host): copy streams, ping-pong staging, ordering events
   cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
-  void* h_in8[2] = {nullptr, nullptr};             // uint8 staging of csnet_plan_run_host_u8
+  void* h_in8[2] = {nullptr, nullptr};             // uint8 staging of csnet_plan_run_host_u8 / _images_u8
   void* h_out8[2] = {nullptr, nullptr};
-  size_t h_in8_bytes = 0;
+  size_t h_in8_bytes = 0, h_out8_bytes = 0;
+  csnet_image_geom* h_geom = nullptr;              // csnet_plan_run_host_images_u8: the batch's geometry, rebased per chunk
+  int32_t h_geom_n = 0;
   void* h_in[2] = {nullptr, nullptr};
   void* h_out[2] = {nullptr, nullptr};
   size_t h_in_bytes = 0, h_out_bytes = 0;
@@ -1271,23 +1275,90 @@ void csnet_plan_destroy(csnet_plan* P) {
     if (P->ev_comp[b]) cudaEventDestroy(P->ev_comp[b]);
     if (P->ev_d2h[b]) cudaEventDestroy(P->ev_d2h[b]);
   }
+  if (P->h_geom) cudaFree(P->h_geom);
   if (P->s_h2d) cudaStreamDestroy(P->s_h2d);
   if (P->s_d2h) cudaStreamDestroy(P->s_d2h);
   delete P;
 }
 
-static int run_host_impl(csnet_plan* P, int32_t N, const void* x_host, void* y_host, void* stream_, bool u8, const float* mean, const float* stdv);
+// What the host buffers of a csnet_plan_run_host* call hold: fp32 tensors, uint8 images at the network size, or packed uint8
+// images of any size with their geometry.
+enum class HostIo { F32, U8, Images };
+struct HostImages {
+  const csnet_image_geom* geom;
+  int64_t x_bytes, y_bytes;
+};
+
+static int run_host_impl(csnet_plan* P, int32_t N, const void* x_host, void* y_host, void* stream_, HostIo io, const float* mean,
+                         const float* stdv, const HostImages* im = nullptr);
 
 int csnet_plan_run_host(csnet_plan* P, int32_t N, const float* x_host, float* y_host, void* stream_) {
-  return run_host_impl(P, N, x_host, y_host, stream_, false, nullptr, nullptr);
+  return run_host_impl(P, N, x_host, y_host, stream_, HostIo::F32, nullptr, nullptr);
 }
 
 int csnet_plan_run_host_u8(csnet_plan* P, int32_t N, const uint8_t* x_hwc, uint8_t* y_u8, const float* mean, const float* stdv, void* stream_) {
   if (!mean || !stdv) return fail(CSNET_E_INVALID, "null mean / std");
-  return run_host_impl(P, N, x_hwc, y_u8, stream_, true, mean, stdv);
+  return run_host_impl(P, N, x_hwc, y_u8, stream_, HostIo::U8, mean, stdv);
 }
 
-static int run_host_impl(csnet_plan* P, int32_t N, const void* x_host, void* y_host, void* stream_, bool u8, const float* mean, const float* stdv) {
+int csnet_plan_run_host_images_u8(csnet_plan* P, int32_t N, const uint8_t* x_packed, int64_t x_bytes, const csnet_image_geom* geom,
+                                  uint8_t* y_packed, int64_t y_bytes, const float* mean, const float* stdv, void* stream_) {
+  if (!geom || !mean || !stdv) return fail(CSNET_E_INVALID, "null geometry / mean / std");
+  const HostImages im{geom, x_bytes, y_bytes};
+  return run_host_impl(P, N, x_packed, y_packed, stream_, HostIo::Images, mean, stdv, &im);
+}
+
+int csnet_resize_u8_to_input(const uint8_t* x_packed, const csnet_image_geom* geom, int32_t N, int32_t H, int32_t W, const float* mean,
+                             const float* stdv, float* x_nchw, void* stream) {
+  if (!x_packed || !geom || !mean || !stdv || !x_nchw) return fail(CSNET_E_INVALID, "csnet_resize_u8_to_input: null argument");
+  if (N <= 0 || N > 65535 || H <= 0 || W <= 0) return fail(CSNET_E_INVALID, "csnet_resize_u8_to_input: N outside [1, 65535] or empty H x W");
+  csnet::launch_resize_in(x_packed, geom, N, H, W, csnet::img_norm(mean, stdv), x_nchw, (cudaStream_t)stream);
+  CU_CHECK(cudaGetLastError());
+  return CSNET_OK;
+}
+
+int csnet_resize_logits_to_u8(const float* logits, int32_t N, int32_t H, int32_t W, const csnet_image_geom* geom, uint8_t* y_packed,
+                              void* stream) {
+  if (!logits || !geom || !y_packed) return fail(CSNET_E_INVALID, "csnet_resize_logits_to_u8: null argument");
+  if (N <= 0 || N > 65535 || H <= 0 || W <= 0) return fail(CSNET_E_INVALID, "csnet_resize_logits_to_u8: N outside [1, 65535] or empty H x W");
+  int dev = 0, sms = 0;
+  CU_CHECK(cudaGetDevice(&dev));
+  CU_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  csnet::launch_resize_out(logits, N, H, W, geom, y_packed, sms, (cudaStream_t)stream);
+  CU_CHECK(cudaGetLastError());
+  return CSNET_OK;
+}
+
+// csnet_plan_run_host_images_u8's geometry, checked before anything is copied or launched.
+static int check_images(const csnet_image_geom* g, int32_t N, int64_t x_bytes, int64_t y_bytes) {
+  for (int32_t i = 0; i < N; ++i) {
+    auto bad = [&](const char* why) { return fail(CSNET_E_INVALID, "run_host_images_u8: image " + std::to_string(i) + why); };
+    if (g[i].h < 1 || g[i].w < 1 || g[i].h > csnet::kMaxImageSide || g[i].w > csnet::kMaxImageSide) return bad(": h or w outside [1, 32767]");
+    const int64_t hw = (int64_t)g[i].h * g[i].w;
+    if (g[i].src_off < 0 || g[i].src_off > x_bytes - 3 * hw) return bad(" lies outside the input buffer");
+    if (g[i].dst_off < 0 || g[i].dst_off > y_bytes - hw) return bad(": its map lies outside the output buffer");
+    if (i > 0 && g[i].dst_off != g[i - 1].dst_off + (int64_t)g[i - 1].h * g[i - 1].w)
+      return bad(": its map does not start where the previous one ends");
+  }
+  return CSNET_OK;
+}
+
+// Ping-pong staging pair that only ever grows.
+static cudaError_t grow_staging(void* (&buf)[2], size_t& bytes, size_t need) {
+  if (need <= bytes) return cudaSuccess;
+  bytes = 0;
+  for (int b = 0; b < 2; ++b) {
+    if (buf[b]) cudaFree(buf[b]);
+    buf[b] = nullptr;
+    const cudaError_t e = cudaMalloc(&buf[b], need);
+    if (e != cudaSuccess) return e;
+  }
+  bytes = need;
+  return cudaSuccess;
+}
+
+static int run_host_impl(csnet_plan* P, int32_t N, const void* x_host, void* y_host, void* stream_, HostIo io, const float* mean,
+                         const float* stdv, const HostImages* im) {
   if (!P || !x_host || !y_host) return fail(CSNET_E_INVALID, "null argument");
   if (N <= 0 || N > P->max_batch) return fail(CSNET_E_INVALID, "batch size outside [1, max_batch]");
   if (P->n_ext != 2) return fail(CSNET_E_INVALID, "run_host needs a plan with externals {0: input, 1: logits}");
@@ -1298,6 +1369,13 @@ static int run_host_impl(csnet_plan* P, int32_t N, const void* x_host, void* y_h
   }
   if (!in || !lo || in->dtype != CSNET_F32 || lo->dtype != CSNET_F32)
     return fail(CSNET_E_INVALID, "run_host: externals must be fp32");
+  if (io != HostIo::F32 && in->C != 3) return fail(CSNET_E_INVALID, "run_host_u8: the network input must have 3 channels");
+  if (io == HostIo::Images) {
+    if (lo->C != 1) return fail(CSNET_E_INVALID, "run_host_images_u8: the logits must have 1 channel");
+    if (N > 65535) return fail(CSNET_E_INVALID, "run_host_images_u8: more than 65535 images");
+    const int rc = check_images(im->geom, N, im->x_bytes, im->y_bytes);
+    if (rc != CSNET_OK) return rc;
+  }
   cudaStream_t stream = (cudaStream_t)stream_;
   DeviceGuard guard_(P->device);
   // The batch is cut into chunks that flow through a three-stage pipeline: H2D copy (own stream) -> program
@@ -1308,7 +1386,10 @@ static int run_host_impl(csnet_plan* P, int32_t N, const void* x_host, void* y_h
   // middle chunk that keeps the kernels at large-batch efficiency.  The uint8 form's copies are 4x smaller: one chunk.
   // Measured at bs 256: fp32 32 / 192 / 32 16.5 ms (4 equal chunks 25.2 ms, 2 equal 24.5 ms, ramps of 4-6 chunks 17.3-20.0 ms);
   // uint8 one chunk 14.7 ms (32 / 192 / 32 16.1 ms).
-  const int edge = N < 64 || u8 ? 0 : N * 32 / 256;
+  // Ragged images run the fp32 schedule: their copies scale with the images, not with the network size.  Measured at bs 256,
+  // h, w in [180, 520] (91 MB in, 30 MB out), fp16 csnet-L-x2 at 224x224 on an H100 80GB HBM3 at 700 W: 32 / 192 / 32 19.60 /
+  // 19.47 ms, one chunk 19.79 / 18.91 ms; the same within the spread, and the edge chunks bound the exposed copies for larger images.
+  const int edge = N < 64 || io == HostIo::U8 ? 0 : N * 32 / 256;
   int sizes[3], n_sizes = 0;
   if (edge > 0) sizes[n_sizes++] = edge;
   sizes[n_sizes++] = N - 2 * edge;
@@ -1336,41 +1417,79 @@ static int run_host_impl(csnet_plan* P, int32_t N, const void* x_host, void* y_h
     P->h_out_bytes = (size_t)chunk * yout;
   }
   const size_t xin8 = xin / sizeof(float), yout8 = yout / sizeof(float);      // bytes per image of the uint8 forms
-  if (u8 && P->h_in8_bytes < (size_t)chunk * xin8) {
-    for (int b = 0; b < 2; ++b) {
-      if (P->h_in8[b]) cudaFree(P->h_in8[b]);
-      if (P->h_out8[b]) cudaFree(P->h_out8[b]);
-      CU_CHECK(cudaMalloc(&P->h_in8[b], (size_t)chunk * xin8));
-      CU_CHECK(cudaMalloc(&P->h_out8[b], (size_t)chunk * yout8));
+  // uint8 staging: the largest chunk's bytes.  Ragged images: the largest byte range that one chunk's images (maps) cover in the
+  // packed input (output); each chunk copies its range, and its geometry is rebased to the staging buffers.
+  size_t in8 = io == HostIo::U8 ? (size_t)chunk * xin8 : 0, out8 = io == HostIo::U8 ? (size_t)chunk * yout8 : 0;
+  int64_t x_lo[3] = {}, x_len[3] = {}, y_lo[3] = {}, y_len[3] = {};
+  std::vector<csnet_image_geom> geom;
+  if (io == HostIo::Images) {
+    geom.assign(im->geom, im->geom + N);
+    for (int it = 0, n0 = 0; it < n_sizes; n0 += sizes[it], ++it) {
+      const int n1 = n0 + sizes[it];
+      int64_t a = INT64_MAX, z = 0;
+      for (int n = n0; n < n1; ++n) {
+        const int64_t s = geom[n].src_off, e = s + 3 * (int64_t)geom[n].h * geom[n].w;
+        a = s < a ? s : a;
+        z = e > z ? e : z;
+      }
+      x_lo[it] = a;
+      x_len[it] = z - a;
+      y_lo[it] = geom[n0].dst_off;
+      y_len[it] = geom[n1 - 1].dst_off + (int64_t)geom[n1 - 1].h * geom[n1 - 1].w - y_lo[it];
+      for (int n = n0; n < n1; ++n) { geom[n].src_off -= x_lo[it]; geom[n].dst_off -= y_lo[it]; }
+      in8 = (size_t)x_len[it] > in8 ? (size_t)x_len[it] : in8;
+      out8 = (size_t)y_len[it] > out8 ? (size_t)y_len[it] : out8;
     }
-    P->h_in8_bytes = (size_t)chunk * xin8;
   }
-  if (u8 && in->C != 3) return fail(CSNET_E_INVALID, "run_host_u8: the network input must have 3 channels");
+  CU_CHECK(grow_staging(P->h_in8, P->h_in8_bytes, in8));
+  CU_CHECK(grow_staging(P->h_out8, P->h_out8_bytes, out8));
+  if (io == HostIo::Images) {
+    if (P->h_geom_n < N) {
+      if (P->h_geom) cudaFree(P->h_geom);
+      P->h_geom = nullptr;
+      P->h_geom_n = 0;
+      CU_CHECK(cudaMalloc(&P->h_geom, (size_t)N * sizeof(csnet_image_geom)));
+      P->h_geom_n = N;
+    }
+    // every chunk's rebased geometry in one upload, ahead of the first chunk's images on the same stream
+    CU_CHECK(cudaMemcpyAsync(P->h_geom, geom.data(), (size_t)N * sizeof(csnet_image_geom), cudaMemcpyHostToDevice, P->s_h2d));
+  }
   PreArgs PA{};
-  if (u8) for (int c = 0; c < 3; ++c) { PA.mean[c] = (double)mean[c]; PA.std[c] = (double)stdv[c]; }
+  if (io == HostIo::U8) for (int c = 0; c < 3; ++c) { PA.mean[c] = (double)mean[c]; PA.std[c] = (double)stdv[c]; }
+  const csnet::ImgNorm IA = io == HostIo::Images ? csnet::img_norm(mean, stdv) : csnet::ImgNorm{};
   int rc = CSNET_OK;
   for (int it = 0, n0 = 0; it < n_sizes && rc == CSNET_OK; n0 += sizes[it], ++it) {
     const int b = it & 1, nb = sizes[it];
     if (it >= 2) CU_CHECK(cudaStreamWaitEvent(P->s_h2d, P->ev_comp[b], 0));     // staging input b was consumed
-    if (u8) CU_CHECK(cudaMemcpyAsync(P->h_in8[b], (const uint8_t*)x_host + (size_t)n0 * xin8, (size_t)nb * xin8, cudaMemcpyHostToDevice, P->s_h2d));
+    if (io == HostIo::U8) CU_CHECK(cudaMemcpyAsync(P->h_in8[b], (const uint8_t*)x_host + (size_t)n0 * xin8, (size_t)nb * xin8, cudaMemcpyHostToDevice, P->s_h2d));
+    else if (io == HostIo::Images) CU_CHECK(cudaMemcpyAsync(P->h_in8[b], (const uint8_t*)x_host + x_lo[it], (size_t)x_len[it], cudaMemcpyHostToDevice, P->s_h2d));
     else CU_CHECK(cudaMemcpyAsync(P->h_in[b], (const float*)x_host + (size_t)n0 * (xin / sizeof(float)), (size_t)nb * xin, cudaMemcpyHostToDevice, P->s_h2d));
     CU_CHECK(cudaEventRecord(P->ev_h2d[b], P->s_h2d));
     CU_CHECK(cudaStreamWaitEvent(stream, P->ev_h2d[b], 0));
     if (it >= 2) CU_CHECK(cudaStreamWaitEvent(stream, P->ev_d2h[b], 0));         // staging output b was drained
-    if (u8) {
+    if (io == HostIo::U8) {
       const int64_t npix = (int64_t)nb * in->H * in->W;
       pre_u8_kernel<<<(unsigned)((npix + kThreads - 1) / kThreads), kThreads, 0, stream>>>((const uint8_t*)P->h_in8[b], (float*)P->h_in[b], npix, (int64_t)in->H * in->W, PA);
+    }
+    if (io == HostIo::Images) {
+      csnet::launch_resize_in((const uint8_t*)P->h_in8[b], P->h_geom + n0, nb, in->H, in->W, IA, (float*)P->h_in[b], stream);
+      CU_CHECK(cudaGetLastError());
     }
     const void* ext[2] = {P->h_in[b], P->h_out[b]};
     rc = run_ops(P, nb, ext, stream);               // (its own staging: no graph path)
     if (rc != CSNET_OK) break;
-    if (u8) {
+    if (io == HostIo::U8) {
       const int64_t nel = (int64_t)nb * lo->C * lo->H * lo->W;
       post_u8_kernel<<<(unsigned)((nel / 4 + kThreads - 1) / kThreads), kThreads, 0, stream>>>((const float*)P->h_out[b], (uint8_t*)P->h_out8[b], nel);
     }
+    if (io == HostIo::Images) {
+      csnet::launch_resize_out((const float*)P->h_out[b], nb, lo->H, lo->W, P->h_geom + n0, (uint8_t*)P->h_out8[b], P->num_sms, stream);
+      CU_CHECK(cudaGetLastError());
+    }
     CU_CHECK(cudaEventRecord(P->ev_comp[b], stream));
     CU_CHECK(cudaStreamWaitEvent(P->s_d2h, P->ev_comp[b], 0));
-    if (u8) CU_CHECK(cudaMemcpyAsync((uint8_t*)y_host + (size_t)n0 * yout8, P->h_out8[b], (size_t)nb * yout8, cudaMemcpyDeviceToHost, P->s_d2h));
+    if (io == HostIo::U8) CU_CHECK(cudaMemcpyAsync((uint8_t*)y_host + (size_t)n0 * yout8, P->h_out8[b], (size_t)nb * yout8, cudaMemcpyDeviceToHost, P->s_d2h));
+    else if (io == HostIo::Images) CU_CHECK(cudaMemcpyAsync((uint8_t*)y_host + y_lo[it], P->h_out8[b], (size_t)y_len[it], cudaMemcpyDeviceToHost, P->s_d2h));
     else CU_CHECK(cudaMemcpyAsync((float*)y_host + (size_t)n0 * (yout / sizeof(float)), P->h_out[b], (size_t)nb * yout, cudaMemcpyDeviceToHost, P->s_d2h));
     CU_CHECK(cudaEventRecord(P->ev_d2h[b], P->s_d2h));
   }

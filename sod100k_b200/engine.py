@@ -5,6 +5,7 @@ from __future__ import annotations
 import os
 from typing import Dict, Tuple
 
+import numpy as np
 import torch
 
 from . import compiler, ir, runtime
@@ -55,6 +56,7 @@ class ModelEngine:
         self._plan_version: Dict[Tuple, int] = {}
         self.frozen = False
         self._epoch = 0
+        self._pinned_images = None          # forward_images_u8's packed host input, reused across calls
 
     def set_precision(self, dtype: str):
         if dtype not in ir.DTYPE_NAMES:
@@ -151,3 +153,55 @@ class ModelEngine:
             out = torch.empty((N, H, W), dtype=torch.uint8, pin_memory=True)
         plan.run_host_u8(N, x_u8.data_ptr(), out.data_ptr(), mean, std, torch.cuda.current_stream(dev).cuda_stream)
         return out
+
+    @staticmethod
+    def _image_u8(im, i: int) -> torch.Tensor:
+        if isinstance(im, np.ndarray):
+            im = torch.from_numpy(np.ascontiguousarray(im))
+        if not isinstance(im, torch.Tensor) or im.dtype != torch.uint8 or im.dim() != 3 or im.shape[2] != 3:
+            raise ValueError(f"image {i}: expected a uint8 [h, w, 3] array or tensor, got "
+                             f"{getattr(im, 'dtype', type(im).__name__)} {tuple(getattr(im, 'shape', ()))}")
+        if not (1 <= im.shape[0] <= 32767 and 1 <= im.shape[1] <= 32767):
+            raise ValueError(f"image {i}: h and w must lie in [1, 32767], got {tuple(im.shape[:2])}")
+        return im.contiguous()
+
+    def forward_images_u8(self, images, size=(224, 224), device: int = 0, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+        """CSNet/test.py:71-98 for a batch of images of any sizes, both skimage resizes included: each uint8 [h, w, 3] image is
+        resized to `size` (skimage >= 0.19 `resize(..., mode='reflect', anti_aliasing=False)`), normalised, run through the network,
+        and its sigmoid map resized back to (h, w) and quantised to uint8.  Returns the uint8 [h_i, w_i] maps in input order.
+
+        `images` are numpy arrays or CPU tensors (the host path: packed into a pinned buffer that is reused across calls, one
+        synchronised C call on plan `device`, the maps are views of one pinned buffer) or all CUDA tensors on one device (the
+        device path: the resizes run around the network on the current stream, no host copies of pixels or maps)."""
+        imgs = [self._image_u8(im, i) for i, im in enumerate(images)]
+        if not imgs:
+            return []
+        if len({t.device for t in imgs}) > 1:
+            raise ValueError("forward_images_u8 takes host images or CUDA images of one device, not a mix")
+        N, (H, W) = len(imgs), (int(size[0]), int(size[1]))
+        geom = runtime.image_geometry([t.shape[:2] for t in imgs])
+        hw = (geom["h"].astype(np.int64) * geom["w"]).tolist()
+        total = sum(hw)
+        if imgs[0].is_cuda:
+            dev = imgs[0].device
+            plan = self.plan_for(N, H, W, dev)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            x = torch.cat([t.reshape(-1) for t in imgs])
+            g = torch.from_numpy(geom.view(np.uint8)).to(dev)
+            x_in = torch.empty((N, 3, H, W), dtype=torch.float32, device=dev)
+            runtime.resize_u8_to_input(x.data_ptr(), g.data_ptr(), N, H, W, mean, std, x_in.data_ptr(), stream)
+            logits = plan.forward(x_in)
+            y = torch.empty(total, dtype=torch.uint8, device=dev)
+            runtime.resize_logits_to_u8(logits.data_ptr(), N, H, W, g.data_ptr(), y.data_ptr(), stream)
+        else:
+            dev = torch.device("cuda", device)
+            plan = self.plan_for(N, H, W, dev)
+            if self._pinned_images is None or self._pinned_images.numel() < 3 * total:
+                self._pinned_images = torch.empty(3 * total, dtype=torch.uint8, pin_memory=True)
+            x = self._pinned_images[:3 * total]
+            torch.cat([t.reshape(-1) for t in imgs], out=x)
+            y = torch.empty(total, dtype=torch.uint8, pin_memory=True)
+            plan.run_host_images_u8(N, x.data_ptr(), 3 * total, geom, y.data_ptr(), total, mean, std,
+                                    torch.cuda.current_stream(dev).cuda_stream)
+        offs = geom["dst_off"].tolist()
+        return [y[o:o + n].view(t.shape[0], t.shape[1]) for o, n, t in zip(offs, hw, imgs)]

@@ -13,7 +13,7 @@ from . import ir
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libcsnet_b200.so")
-ABI_VERSION = 5
+ABI_VERSION = 6
 PARAM_EPOCH = 0      # bumped by in-place parameter updates that bypass torch's version counters (FusedAdam)
 _lib = None
 
@@ -21,6 +21,7 @@ _lib = None
 SYMBOLS = ("csnet_abi_version", "csnet_last_error", "csnet_device_count", "csnet_plan_create",
            "csnet_plan_set_blob", "csnet_plan_run", "csnet_plan_profile", "csnet_plan_tensor_ptr", "csnet_plan_read_tensor", "csnet_plan_op_kernel", "csnet_plan_launches",
            "csnet_plan_arena_bytes", "csnet_plan_destroy", "csnet_plan_run_host", "csnet_plan_run_host_u8",
+           "csnet_resize_u8_to_input", "csnet_resize_logits_to_u8", "csnet_plan_run_host_images_u8",
            "csnet_train_last_error", "csnet_train_bn_stats", "csnet_train_bn_prelu_fwd", "csnet_train_bn_prelu_bwd",
            "csnet_train_dw_conv", "csnet_train_dw_wgrad", "csnet_train_dw_bwd", "csnet_train_mix_fwd", "csnet_train_mix_dgrad",
            "csnet_train_mix_wgrad", "csnet_train_pool_fwd", "csnet_train_pool_bwd", "csnet_slim_gather", "csnet_train_bce", "csnet_train_adam", "csnet_salmetric_hist")
@@ -28,6 +29,27 @@ SYMBOLS = ("csnet_abi_version", "csnet_last_error", "csnet_device_count", "csnet
 
 class EngineError(RuntimeError):
     pass
+
+
+class ImageGeom(C.Structure):
+    """csnet_image_geom: image i of a ragged batch is uint8 [h][w][3] at byte src_off of the packed input; its map is uint8 [h][w]
+    at byte dst_off of the packed output."""
+    _fields_ = [("src_off", C.c_int64), ("dst_off", C.c_int64), ("h", C.c_int32), ("w", C.c_int32)]
+
+
+assert C.sizeof(ImageGeom) == 24
+GEOM_DTYPE = np.dtype(ImageGeom)
+
+
+def image_geometry(sizes) -> np.ndarray:
+    """Geometry (GEOM_DTYPE [N]) of images of the given (h, w) sizes packed back to back in order, input and output alike."""
+    hw = np.array([(int(h), int(w)) for h, w in sizes], np.int64).reshape(-1, 2)
+    n = hw[:, 0] * hw[:, 1]
+    g = np.zeros(len(n), GEOM_DTYPE)
+    g["dst_off"][1:] = np.cumsum(n)[:-1]
+    g["src_off"] = 3 * g["dst_off"]
+    g["h"], g["w"] = hw[:, 0], hw[:, 1]
+    return g
 
 
 def load_library(path: Optional[str] = None):
@@ -69,6 +91,14 @@ def load_library(path: Optional[str] = None):
     lib.csnet_plan_run_host.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.csnet_plan_run_host_u8.restype = C.c_int
     lib.csnet_plan_run_host_u8.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_void_p]
+    lib.csnet_resize_u8_to_input.restype = C.c_int
+    lib.csnet_resize_u8_to_input.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float),
+                                             C.POINTER(C.c_float), C.c_void_p, C.c_void_p]
+    lib.csnet_resize_logits_to_u8.restype = C.c_int
+    lib.csnet_resize_logits_to_u8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.csnet_plan_run_host_images_u8.restype = C.c_int
+    lib.csnet_plan_run_host_images_u8.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
+                                                  C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_void_p]
     lib.csnet_slim_gather.restype = C.c_int
     lib.csnet_slim_gather.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     lib.csnet_train_last_error.restype = C.c_char_p
@@ -82,6 +112,21 @@ def load_library(path: Optional[str] = None):
 def _check(lib, rc: int, what: str):
     if rc != 0:
         raise EngineError(f"{what} failed ({rc}): {lib.csnet_last_error().decode()}")
+
+
+def resize_u8_to_input(x_packed_ptr: int, geom_dev_ptr: int, N: int, H: int, W: int, mean, std, x_nchw_ptr: int, stream: int = 0):
+    """Device to device: packed uint8 images (geometry on the device) -> fp32 [N,3,H,W] network input (csnet_resize_u8_to_input)."""
+    lib = load_library()
+    m, s_ = (C.c_float * 3)(*mean), (C.c_float * 3)(*std)
+    _check(lib, lib.csnet_resize_u8_to_input(x_packed_ptr, geom_dev_ptr, int(N), int(H), int(W), m, s_, x_nchw_ptr, stream),
+           "csnet_resize_u8_to_input")
+
+
+def resize_logits_to_u8(logits_ptr: int, N: int, H: int, W: int, geom_dev_ptr: int, y_packed_ptr: int, stream: int = 0):
+    """Device to device: fp32 logits [N,1,H,W] -> each image's uint8 map at its dst_off (csnet_resize_logits_to_u8)."""
+    lib = load_library()
+    _check(lib, lib.csnet_resize_logits_to_u8(logits_ptr, int(N), int(H), int(W), geom_dev_ptr, y_packed_ptr, stream),
+           "csnet_resize_logits_to_u8")
 
 
 class Plan:
@@ -125,6 +170,16 @@ class Plan:
     def run_host_u8(self, N: int, x_host_ptr: int, y_host_ptr: int, mean, std, stream: int = 0):
         m, s_ = (C.c_float * 3)(*mean), (C.c_float * 3)(*std)
         _check(self.lib, self.lib.csnet_plan_run_host_u8(self._h, int(N), x_host_ptr, y_host_ptr, m, s_, stream), "csnet_plan_run_host_u8")
+
+    def run_host_images_u8(self, N: int, x_host_ptr: int, x_bytes: int, geom: np.ndarray, y_host_ptr: int, y_bytes: int, mean, std,
+                           stream: int = 0):
+        """Ragged uint8 images (host, packed, `geom`: GEOM_DTYPE [N] on the host) -> uint8 maps at each image's size, synchronised."""
+        geom = np.ascontiguousarray(geom, GEOM_DTYPE)
+        if geom.shape != (int(N),):
+            raise ValueError(f"geometry for {geom.shape} images, batch of {N}")
+        m, s_ = (C.c_float * 3)(*mean), (C.c_float * 3)(*std)
+        _check(self.lib, self.lib.csnet_plan_run_host_images_u8(self._h, int(N), x_host_ptr, int(x_bytes), geom.ctypes.data, y_host_ptr,
+                                                                int(y_bytes), m, s_, stream), "csnet_plan_run_host_images_u8")
 
     def tensor_ptr(self, tensor: int, N: int) -> int:
         return int(self.lib.csnet_plan_tensor_ptr(self._h, tensor, N) or 0)
