@@ -170,7 +170,9 @@ __device__ __forceinline__ void ms_consume_n(const MsArgs& A, uint32_t sbase, ui
   }
 }
 
-template <typename T>
+// PROJ_RS: the instantiation for projected (MIXPROJ) ops that also carry resample-add paths.  It is a kernel of its own so
+// that its consumers do not enlarge the register / spill footprint of the instantiation every other op runs.
+template <typename T, bool PROJ_RS = false>
 __global__ void __launch_bounds__(kMsThreads, 1)
 mix_stream_kernel(const __grid_constant__ MsArgs A, const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
                   const __grid_constant__ CUtensorMap tm2, const __grid_constant__ CUtensorMap tr0, const __grid_constant__ CUtensorMap tr1) {
@@ -266,7 +268,11 @@ mix_stream_kernel(const __grid_constant__ MsArgs A, const __grid_constant__ CUte
   } else if (warp >= 4) {
     const int e = warp - 4, qd = e & 3, wg = e >> 2;
     const uint32_t ready = A.k3 ? bar_built : bar_full;
-    if (A.has_proj) ms_consume_n<T, 0, true>(A, sbase, STG, TAB, bar_full, ready, bar_empty, ra, rb, wg, qd, lane);
+    // a projected op adds its resample paths before the PReLU like any other (the host launches PROJ_RS for those)
+    if constexpr (PROJ_RS) {
+      if (A.n_rs == 1) ms_consume_n<T, 1, true>(A, sbase, STG, TAB, bar_full, ready, bar_empty, ra, rb, wg, qd, lane);
+      else ms_consume_n<T, 2, true>(A, sbase, STG, TAB, bar_full, ready, bar_empty, ra, rb, wg, qd, lane);
+    } else if (A.has_proj) ms_consume_n<T, 0, true>(A, sbase, STG, TAB, bar_full, ready, bar_empty, ra, rb, wg, qd, lane);
     else if (A.n_rs == 0) ms_consume_n<T, 0, false>(A, sbase, STG, TAB, bar_full, ready, bar_empty, ra, rb, wg, qd, lane);
     else if (A.n_rs == 1) ms_consume_n<T, 1, false>(A, sbase, STG, TAB, bar_full, ready, bar_empty, ra, rb, wg, qd, lane);
     else ms_consume_n<T, 2, false>(A, sbase, STG, TAB, bar_full, ready, bar_empty, ra, rb, wg, qd, lane);

@@ -796,7 +796,9 @@ int plan_op(csnet_plan& P, size_t i) {
   cudaError_t e = cudaSuccess;
   switch (R.kern) {
     case Kern::MixStream:
-      e = cudaFuncSetAttribute(csnet::mix_stream_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOptIn);
+      e = R.ms.has_proj && R.ms.n_rs > 0
+              ? cudaFuncSetAttribute(csnet::mix_stream_kernel<__half, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOptIn)
+              : cudaFuncSetAttribute(csnet::mix_stream_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemOptIn);
       break;
     case Kern::MixTc: {
       const int C = mix_channels(P, op), slice = R.tc.mt * 16, m16t = (C + slice - 1) / slice * slice, WR = R.tc.kc + 8;
@@ -1021,7 +1023,10 @@ static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_
       for (int k = A.n_rs; k < csnet::kMsMaxRs; ++k) rmaps[k] = maps[0];
       int grid = A.total_chunks / 2;
       grid = grid < 1 ? 1 : (grid > P->num_sms ? P->num_sms : grid);
-      csnet::mix_stream_kernel<__half><<<grid, csnet::kMsThreads, A.smem_bytes, stream>>>(A, maps[0], maps[1], maps[2], rmaps[0], rmaps[1]);
+      if (A.has_proj && A.n_rs > 0)
+        csnet::mix_stream_kernel<__half, true><<<grid, csnet::kMsThreads, A.smem_bytes, stream>>>(A, maps[0], maps[1], maps[2], rmaps[0], rmaps[1]);
+      else
+        csnet::mix_stream_kernel<__half><<<grid, csnet::kMsThreads, A.smem_bytes, stream>>>(A, maps[0], maps[1], maps[2], rmaps[0], rmaps[1]);
       break;
     }
     case Kern::MixTc: {
