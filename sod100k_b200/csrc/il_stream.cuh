@@ -14,9 +14,9 @@
 //   GEMM       a warpgroup issues wgmma.mma_async (f16 x f16 -> f32, M = 64 pixels, N = ru16(Cout), K = 16 per
 //              instruction) per 8 pixel groups straight from the shared-memory tiles; fp32 accumulators in registers.
 //   epilogue   from the accumulator fragment: + bias, PReLU, 16-bit, written IN PLACE over the chunk (T1).
-//   dw tail    a thread owns (channel, 8-pixel column) for the whole walk and keeps the 3-row windows of T1 and T2
-//              in registers: dw3x3+BN+PReLU twice with no halo recomputation in y, no shared-memory round trip for
-//              T2, 16-byte coalesced stores of the block output.  (mixed-precision FMA: fp16 x fp16 + fp32.)
+//   dw tail    a thread owns (channel, two 8-pixel groups) for the whole walk and keeps the open rows of both 3x3 layers
+//              as fp32 running sums in registers: dw3x3+BN+PReLU twice with no halo recomputation in y, no shared-memory
+//              round trip for T2, 16-byte coalesced stores of the block output.  (mixed-precision FMA: fp16 x fp16 + fp32.)
 //
 // Stem form (kStem; the first block, csnet.py:60-71: both branches are 3x3 convs of the fp32 image, the lo one of its 2x2
 // max-pool): the TMA ring holds 4-row blocks of the fp32 image (4-D map, zero fill outside the image = the conv padding);
@@ -35,7 +35,7 @@
 
 namespace csnet {
 
-constexpr int kIlsMaxThreads = 768;
+constexpr int kIlsMaxThreads = 384;   // 168 registers a thread: the tail's fp32 sums of 16 pixels stay out of local memory
 constexpr int kIlsMaxC = 64;          // output channels per branch (epilogue parameter tables in the kernel arguments)
 constexpr int kIlsHiStages = 2, kIlsLoStages = 3;
 
@@ -56,9 +56,9 @@ struct IlsArgs {
   int32_t Ci, BW;                     // stem form: image channels; width in floats of an image block in shared memory (8 GR + 8)
   int32_t off_xlo;                    // stem form: the lo chunk's GEMM operand buffer
   int32_t cpi, total_chunks;          // chunks per image strip (H/4), N * ns * cpi
-  int32_t dw_warps;                   // warps of the CTA = warps of the depthwise tail (tasks packed: hi columns, then lo)
+  int32_t dw_warps;                   // warps of the CTA = warps of the depthwise tail (tasks packed: hi group pairs, then lo)
   int32_t hi_stage_bytes, lo_stage_bytes;
-  int32_t off_xl, off_xh, off_t1l, off_wbh, off_wbl, off_bar, off_zero, off_epi, smem_bytes;
+  int32_t off_xl, off_xh, off_t1l, off_wbh, off_wbl, off_bar, off_zero, off_epi, off_dwp, smem_bytes;
 };
 
 __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2, int c3, int c4) {
@@ -91,6 +91,8 @@ __device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes
 }
 // wgmma.m64nNk16, fp32 += f16 x f16: A (64 pixels x 16 channels) MN-major from shared memory (transposed: pixels are the
 // contiguous dimension of a core matrix), B (N output channels x 16) K-major; d: the warpgroup's accumulator fragment.
+// mma0 starts a group (scale-d = 0, d write-only): no other instruction defines the accumulator registers before the MMAs,
+// which would make ptxas serialize the group's wgmmas.
 template <int N> struct Wgmma;
 template <> struct Wgmma<16> {
   static __device__ __forceinline__ void mma(float (&d)[8], uint64_t da, uint64_t db, uint32_t acc) {
@@ -98,6 +100,12 @@ template <> struct Wgmma<16> {
                  "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 1, 0;\n}\n"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
                  : "l"(da), "l"(db), "r"(acc));
+  }
+  static __device__ __forceinline__ void mma0(float (&d)[8], uint64_t da, uint64_t db) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 1, 0;\n}\n"
+                 : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7])
+                 : "l"(da), "l"(db), "r"(0u));
   }
 };
 template <> struct Wgmma<32> {
@@ -107,6 +115,12 @@ template <> struct Wgmma<32> {
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
                  : "l"(da), "l"(db), "r"(acc));
   }
+  static __device__ __forceinline__ void mma0(float (&d)[16], uint64_t da, uint64_t db) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 1, 0;\n}\n"
+                 : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]), "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15])
+                 : "l"(da), "l"(db), "r"(0u));
+  }
 };
 template <> struct Wgmma<48> {
   static __device__ __forceinline__ void mma(float (&d)[24], uint64_t da, uint64_t db, uint32_t acc) {
@@ -114,6 +128,12 @@ template <> struct Wgmma<48> {
                  "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, 1, 0;\n}\n"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
                  : "l"(da), "l"(db), "r"(acc));
+  }
+  static __device__ __forceinline__ void mma0(float (&d)[24], uint64_t da, uint64_t db) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %26, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, 1, 0;\n}\n"
+                 : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]), "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]), "=f"(d[16]), "=f"(d[17]), "=f"(d[18]), "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23])
+                 : "l"(da), "l"(db), "r"(0u));
   }
 };
 template <> struct Wgmma<64> {
@@ -123,6 +143,12 @@ template <> struct Wgmma<64> {
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
                  : "l"(da), "l"(db), "r"(acc));
   }
+  static __device__ __forceinline__ void mma0(float (&d)[32], uint64_t da, uint64_t db) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 1, 0;\n}\n"
+                 : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]), "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]), "=f"(d[16]), "=f"(d[17]), "=f"(d[18]), "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23]), "=f"(d[24]), "=f"(d[25]), "=f"(d[26]), "=f"(d[27]), "=f"(d[28]), "=f"(d[29]), "=f"(d[30]), "=f"(d[31])
+                 : "l"(da), "l"(db), "r"(0u));
+  }
 };
 template <> struct Wgmma<80> {
   static __device__ __forceinline__ void mma(float (&d)[40], uint64_t da, uint64_t db, uint32_t acc) {
@@ -130,6 +156,12 @@ template <> struct Wgmma<80> {
                  "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 1, 0;\n}\n"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
                  : "l"(da), "l"(db), "r"(acc));
+  }
+  static __device__ __forceinline__ void mma0(float (&d)[40], uint64_t da, uint64_t db) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %42, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 1, 0;\n}\n"
+                 : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]), "=f"(d[8]), "=f"(d[9]), "=f"(d[10]), "=f"(d[11]), "=f"(d[12]), "=f"(d[13]), "=f"(d[14]), "=f"(d[15]), "=f"(d[16]), "=f"(d[17]), "=f"(d[18]), "=f"(d[19]), "=f"(d[20]), "=f"(d[21]), "=f"(d[22]), "=f"(d[23]), "=f"(d[24]), "=f"(d[25]), "=f"(d[26]), "=f"(d[27]), "=f"(d[28]), "=f"(d[29]), "=f"(d[30]), "=f"(d[31]), "=f"(d[32]), "=f"(d[33]), "=f"(d[34]), "=f"(d[35]), "=f"(d[36]), "=f"(d[37]), "=f"(d[38]), "=f"(d[39])
+                 : "l"(da), "l"(db), "r"(0u));
   }
 };
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
@@ -141,10 +173,9 @@ __device__ __forceinline__ void warpgroup_bar(int wg) { asm volatile("bar.sync %
 // One 64-pixel block of the warpgroup: d = A[64][K16] . B[N][K16]^T over K16 / 16 instructions.
 template <int N>
 __device__ __forceinline__ void wgmma_block(float (&d)[N / 2], uint64_t da, uint64_t db, int K16) {
-#pragma unroll
-  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
   wgmma_fence();
-  for (int ks = 0; ks < (K16 >> 4); ++ks) Wgmma<N>::mma(d, da + (uint64_t)(16 * ks), db + (uint64_t)(16 * ks), ks > 0);
+  Wgmma<N>::mma0(d, da, db);
+  for (int ks = 1; ks < (K16 >> 4); ++ks) Wgmma<N>::mma(d, da + (uint64_t)(16 * ks), db + (uint64_t)(16 * ks), 1u);
   wgmma_commit_wait();
 }
 __device__ __forceinline__ uint32_t lds32(uint32_t a) { uint32_t v; asm volatile("ld.shared.b32 %0, [%1];\n" : "=r"(v) : "r"(a)); return v; }
@@ -163,60 +194,98 @@ __device__ __forceinline__ void sts16(uint32_t a, uint16_t v) { asm volatile("st
 // element j of a row of packed 16-bit pairs
 __device__ __forceinline__ uint16_t h16(const uint32_t* row, int j) { return (j & 1) ? (uint16_t)(row[j >> 1] >> 16) : (uint16_t)row[j >> 1]; }
 
-// One step of the depthwise tail: T1 row r arrives (n1: pixels x0-2 .. x0+9 of this thread's channel), T2 row r-1 is
-// made from T1 rows r-2, r-1, r (10 pixels: x0-1 .. x0+8), the block output row r-2 from T2 rows r-3, r-2, r-1.
+// The depthwise tail.  A thread owns one channel and two 8-pixel groups A, B (x0 .. x0+15) of a strip row for the whole
+// walk and keeps running sums instead of windows of its inputs: a 3x3 output row is finished by its third input row, so per
+// layer the thread holds the two output rows still open (one started by one input row, one by two).  Each input value is
+// converted to fp32 once, when its row arrives, and every sum still runs  bias, taps dy = 0, 1, 2 (dx = 0, 1, 2 within)  in
+// that order: the chain of the mixed-precision FMA (fp16 x fp16 + fp32), operand for operand.
+// Parameters: per tail channel in shared memory, for dw1 then dw2, three float4 {3 weights of tap row dy (rounded through
+// the 16-bit type), x}, x = bias, slope - 1, 0: one 16-byte load right before each tap row is used.
+constexpr int kIlsDwpBytes = 96;
+constexpr int kIlsTX = 20, kIlsT2 = 18, kIlsTO = 16;   // a T1 row of a task (x0-2 .. x0+17), its T2 row (x0-1 .. x0+16), output
+
+// acc[i] += row[i + dx] * w[dx], dx = 0, 1, 2 (one tap row of a 3x3 over NO outputs); kStart: acc[i] = w.w (the bias) first
+template <int NO, bool kStart = false>
+__device__ __forceinline__ void ils_dw_taps(float (&acc)[NO], const float* row, float4 w) {
+#pragma unroll
+  for (int i = 0; i < NO; ++i) {
+    acc[i] = fmaf(row[i], w.x, kStart ? w.w : acc[i]);
+    acc[i] = fmaf(row[i + 1], w.y, acc[i]);
+    acc[i] = fmaf(row[i + 2], w.z, acc[i]);
+  }
+}
+__device__ __forceinline__ float4 ils_dw_param(uint32_t a) {
+  const uint4 v = lds128(a);
+  return make_float4(__uint_as_float(v.x), __uint_as_float(v.y), __uint_as_float(v.z), __uint_as_float(v.w));
+}
+struct IlsTail {
+  float s2a[kIlsT2], s2b[kIlsT2];    // T2 rows r-1 (two input rows in), r (one)
+  float soa[kIlsTO], sob[kIlsTO];    // output rows r-2 (two T2 rows in), r-1 (one)
+};
+// The sums of a walk's start: the rows above its first T1 row are zero (as if the windows started from zero).  The zero
+// is opaque to the compiler: folding 0 * w + acc to acc would differ for a -0 bias or a non-finite weight.
+__device__ __forceinline__ void ils_dw_start(IlsTail& t, uint32_t prm) {
+  float z0;
+  asm("mov.b32 %0, 0;\n" : "=f"(z0));
+  float z[kIlsTX];
+#pragma unroll
+  for (int i = 0; i < kIlsTX; ++i) z[i] = z0;
+  float4 w0 = ils_dw_param(prm), w1 = ils_dw_param(prm + 16u);
+  ils_dw_taps<kIlsT2, true>(t.s2a, z, w0); ils_dw_taps<kIlsT2>(t.s2a, z, w1); ils_dw_taps<kIlsT2, true>(t.s2b, z, w0);
+  w0 = ils_dw_param(prm + 48u); w1 = ils_dw_param(prm + 64u);
+  ils_dw_taps<kIlsTO, true>(t.soa, z, w0); ils_dw_taps<kIlsTO>(t.soa, z, w1); ils_dw_taps<kIlsTO, true>(t.sob, z, w0);
+}
+// Per-task constants of the tail: T2 at x0-1, x0+8, x0+16 is conv padding (x 0) at the image's edges; B may lie past the
+// strip (its outputs are not stored) or past the image (zeros).
+struct IlsTaskEdges {
+  float m0, m9, m17;
+  bool outB;
+};
+// One step: T1 row r arrives (x) and finishes T2 row r-1 (s2a), which finishes the block output row r-2 (soa).  On return
+// s2a / soa hold the rows just started (T2 row r+1, output row r); s2b / sob swap roles with them: the caller passes the
+// sums of even and odd rows in turn (a = s2a/soa, b = s2b/sob of the row).
 template <typename T>
-__device__ __forceinline__ void ils_dw_push(uint32_t (&t1)[2][6], uint32_t (&t2)[2][5], const uint32_t (&n1)[6],
-                                            const uint32_t (&w1)[5], float b1, float s1, const uint32_t (&w2)[5], float b2, float s2,
-                                            bool make_t2, float mL, float mR, bool make_out, uint16_t* out) {
-  uint32_t q[5];
-  if (make_t2) {
+__device__ __forceinline__ void ils_dw_push(float (&s2a)[kIlsT2], float (&s2b)[kIlsT2], float (&soa)[kIlsTO], float (&sob)[kIlsTO],
+                                            const float (&x)[kIlsTX], uint32_t prm, bool make_t2, const IlsTaskEdges& e, bool make_out,
+                                            uint16_t* out) {
+  ils_dw_taps<kIlsT2>(s2a, x, ils_dw_param(prm + 32u));
+  const float4 w1 = ils_dw_param(prm + 16u);
+  float q[kIlsT2];                   // T2 row r-1, rounded through the 16-bit type (zero: conv padding / not needed)
 #pragma unroll
-    for (int i = 0; i < 10; i += 2) {
-      float v0 = b1, v1 = b1;
-#pragma unroll
-      for (int dy = 0; dy < 3; ++dy) {
-        const uint32_t* row = dy == 0 ? t1[0] : (dy == 1 ? t1[1] : n1);
-#pragma unroll
-        for (int dx = 0; dx < 3; ++dx) {
-          const uint16_t w = h16(w1, dy * 3 + dx);
-          v0 = Pack<T>::fma16(h16(row, i + dx), w, v0);
-          v1 = Pack<T>::fma16(h16(row, i + 1 + dx), w, v1);
-        }
-      }
-      v0 = prelu_m1(v0, s1);
-      v1 = prelu_m1(v1, s1);
-      if (i == 0) v0 *= mL;          // T2 at x0-1 is conv padding when the column is the image's first
-      if (i == 8) v1 *= mR;          // T2 at x0+8 likewise on the right
-      q[i >> 1] = Pack<T>::from_f2(v0, v1);
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 5; ++i) q[i] = 0u;
+  for (int i = 0; i < kIlsT2; i += 2) {
+    float v0 = prelu_m1(s2a[i], w1.w), v1 = prelu_m1(s2a[i + 1], w1.w);
+    if (i == 0) v0 *= e.m0;
+    if (i == 8) v1 *= e.m9;
+    if (i == 16) v1 *= e.m17;
+    const float2 r = Pack<T>::to_f2(Pack<T>::from_f2(v0, v1));
+    q[i] = make_t2 ? r.x : 0.f;
+    q[i + 1] = make_t2 ? r.y : 0.f;
   }
+  ils_dw_taps<kIlsT2>(s2b, x, w1);
+  ils_dw_taps<kIlsTO>(soa, q, ils_dw_param(prm + 80u));
+  const float4 v1 = ils_dw_param(prm + 64u);
+  ils_dw_taps<kIlsTO>(sob, q, v1);
   if (make_out) {
-    uint32_t o[4];
+    uint32_t o[8];
 #pragma unroll
-    for (int k = 0; k < 8; k += 2) {
-      float v0 = b2, v1 = b2;
-#pragma unroll
-      for (int dy = 0; dy < 3; ++dy) {
-        const uint32_t* row = dy == 0 ? t2[0] : (dy == 1 ? t2[1] : q);
-#pragma unroll
-        for (int dx = 0; dx < 3; ++dx) {
-          const uint16_t w = h16(w2, dy * 3 + dx);
-          v0 = Pack<T>::fma16(h16(row, k + dx), w, v0);
-          v1 = Pack<T>::fma16(h16(row, k + 1 + dx), w, v1);
-        }
-      }
-      o[k >> 1] = Pack<T>::from_f2(prelu_m1(v0, s2), prelu_m1(v1, s2));
-    }
+    for (int k = 0; k < kIlsTO; k += 2) o[k >> 1] = Pack<T>::from_f2(prelu_m1(soa[k], v1.w), prelu_m1(soa[k + 1], v1.w));
     *reinterpret_cast<uint4*>(out) = make_uint4(o[0], o[1], o[2], o[3]);
+    if (e.outB) *reinterpret_cast<uint4*>(out + 8) = make_uint4(o[4], o[5], o[6], o[7]);
   }
+  ils_dw_taps<kIlsTO, true>(soa, q, ils_dw_param(prm + 48u));
+  ils_dw_taps<kIlsT2, true>(s2a, x, ils_dw_param(prm));
+}
+// A T1 row of the tail from shared memory, converted to fp32: pA = group A's 16 bytes, pB = group B's (or zeros), pL / pR
+// the neighbour groups' edge pairs (or zeros at the image's edges).
+template <typename T>
+__device__ __forceinline__ void ils_dw_load(float (&x)[kIlsTX], uint32_t pA, uint32_t pB, uint32_t pL, uint32_t pR) {
+  const uint4 a = lds128(pA), b = lds128(pB);
+  const uint32_t u[10] = {lds32(pL), a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w, lds32(pR)};
 #pragma unroll
-  for (int i = 0; i < 6; ++i) { t1[0][i] = t1[1][i]; t1[1][i] = n1[i]; }
-#pragma unroll
-  for (int i = 0; i < 5; ++i) { t2[0][i] = t2[1][i]; t2[1][i] = q[i]; }
+  for (int i = 0; i < 10; ++i) {
+    const float2 f = Pack<T>::to_f2(u[i]);
+    x[2 * i] = f.x; x[2 * i + 1] = f.y;
+  }
 }
 
 __device__ __forceinline__ void stsm_x4_trans(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
@@ -323,38 +392,36 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
       float* ep = reinterpret_cast<float*>(gbase + A.off_epi);
       ep[tid] = A.bias_h[tid]; ep[kIlsMaxC + tid] = A.sm1_h[tid]; ep[2 * kIlsMaxC + tid] = A.bias_l[tid]; ep[3 * kIlsMaxC + tid] = A.sm1_l[tid];
     }
+    // depthwise-tail parameter records: hi channels, then lo ones
+    float* dp = reinterpret_cast<float*>(gbase + A.off_dwp);
+    for (int i = tid; i < (Cho + Clo) * 24; i += nthreads) {
+      const int ch = i / 24, j = i - ch * 24, lyr = j / 12, dy = (j >> 2) % 3, k = j & 3;
+      const bool hi = ch < Cho;
+      const int cc = hi ? ch : ch - Cho;
+      const DwParams& P = lyr ? (hi ? A.dw2h : A.dw2l) : (hi ? A.dw1h : A.dw1l);
+      float v = 0.f;
+      if (k < 3) v = Pack<T>::to_f2(Pack<T>::from_f2(__ldg(P.w + cc * 9 + dy * 3 + k), 0.f)).x;
+      else if (dy == 0) v = __ldg(P.b + cc);
+      else if (dy == 1) v = __ldg(P.s + cc) - 1.f;
+      dp[i] = v;
+    }
   }
   asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
   __syncthreads();
 
-  // depthwise-tail role of this thread (fixed for the whole kernel): a channel and an 8-pixel column
-  // tail tasks are packed: threads [0, Cho * gsn) own a hi (channel, column), the next Clo * gsn / 2 a lo one
-  const int n_hi_tasks = Cho * gsn;
+  // depthwise-tail role of this thread (fixed for the whole kernel): a channel and two 8-pixel groups of a strip row
+  // tail tasks are packed: threads [0, Cho * gsn / 2) own a hi (channel, group pair), the next Clo * ceil(gsn / 4) a lo one
+  const int n_hi_tasks = Cho * (gsn >> 1);
   const bool dw_hi = tid < n_hi_tasks;
   const int dwt = dw_hi ? tid : tid - n_hi_tasks;
-  const int Gd = dw_hi ? gsn : gsn >> 1, Cd = dw_hi ? Cho : Clo, Sd = dw_hi ? SH : ST;   // Gd: this role's groups per strip row
+  const int Gs = dw_hi ? gsn : gsn >> 1;                  // this role's groups per strip row
+  const int Gd = (Gs + 1) >> 1, Cd = dw_hi ? Cho : Clo, Sd = dw_hi ? SH : ST;   // Gd: tasks per channel of a strip row
   const bool dw_live = dwt < Cd * Gd;
-  const int dc = dw_live ? dwt / Gd : 0, dg = dw_live ? dwt - dc * Gd : 0;
-  uint32_t w1[5], w2[5];
-  float b1, s1, b2, s2;
-  {
-    const DwParams& P1 = dw_hi ? A.dw1h : A.dw1l;
-    const DwParams& P2 = dw_hi ? A.dw2h : A.dw2l;
-    float f1[10], f2[10];
-#pragma unroll
-    for (int i = 0; i < 9; ++i) {
-      f1[i] = dw_live ? __ldg(P1.w + dc * 9 + i) : 0.f;
-      f2[i] = dw_live ? __ldg(P2.w + dc * 9 + i) : 0.f;
-    }
-    f1[9] = f2[9] = 0.f;
-#pragma unroll
-    for (int i = 0; i < 5; ++i) { w1[i] = Pack<T>::from_f2(f1[2 * i], f1[2 * i + 1]); w2[i] = Pack<T>::from_f2(f2[2 * i], f2[2 * i + 1]); }
-    b1 = dw_live ? __ldg(P1.b + dc) : 0.f; s1 = dw_live ? __ldg(P1.s + dc) - 1.f : 0.f;
-    b2 = dw_live ? __ldg(P2.b + dc) : 0.f; s2 = dw_live ? __ldg(P2.s + dc) - 1.f : 0.f;
-  }
+  const int dc = dw_live ? dwt / Gd : 0, dg = dw_live ? 2 * (dwt - dc * Gd) : 0;  // dg: group A in the strip row
+  const uint32_t prm = sbase + A.off_dwp + (uint32_t)((dw_hi ? dc : Cho + dc) * kIlsDwpBytes);
   const int dw_rows = dw_hi ? 4 : 2;                      // T1 rows per chunk of this role
   const int dHd = dw_hi ? H : Hl, dWd = dw_hi ? W : Wl;
-  // byte offsets inside a T1 chunk of this thread's 16-byte row (row 0) and of its two halo pairs
+  // byte offset inside a T1 chunk of group A's 16-byte row (row 0)
   const uint32_t dw_off = (uint32_t)((dg + hl) * Sd + dc) * 16u, dw_rowstep = (uint32_t)((dw_hi ? GR : GLR) * Sd) * 16u;
   const int Gimg = dw_hi ? GH : GL;                       // groups per image row of this role
 
@@ -401,14 +468,18 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
       for (int cl = cl0; cl <= cl1 && cl <= c0 + 1; ++cl) issue_lo(cl);
     }
     int lo_waited = 0;
-    uint32_t t1w[2][6], t2w[2][5];
-#pragma unroll
-    for (int i = 0; i < 6; ++i) t1w[0][i] = t1w[1][i] = 0u;
-#pragma unroll
-    for (int i = 0; i < 5; ++i) t2w[0][i] = t2w[1][i] = 0u;
-    const int gimg = (dw_hi ? gs0 : gs0 >> 1) + dg;                                // this thread's group in the image row
-    const bool edgeL = gimg == 0, edgeR = gimg == Gimg - 1;
-    const float mL = edgeL ? 0.f : 1.f, mR = edgeR ? 0.f : 1.f;
+    IlsTail tl;                                                                    // the tail's open rows (ils_dw_push)
+    if (dw_live) ils_dw_start(tl, prm);
+    const int gimg = (dw_hi ? gs0 : gs0 >> 1) + dg;                                // group A in the image row
+    // group B: in the image (else zeros, T2 at x0+8 is padding); in the strip (else its outputs belong to the next one)
+    // the neighbour pair right of B: zeros past the image, and past the tile (then B is the halo and not stored)
+    const bool hasB = gimg + 1 < Gimg, zeroL = gimg == 0, zeroR = gimg + 2 >= Gimg || dg + 2 >= Gs + hl;
+    IlsTaskEdges edg;
+    edg.m0 = zeroL ? 0.f : 1.f;
+    edg.m9 = hasB ? 1.f : 0.f;
+    edg.m17 = gimg + 2 >= Gimg ? 0.f : 1.f;
+    edg.outB = dg + 1 < Gs;
+    const uint32_t sd = (uint32_t)Sd * 16u;
     uint16_t* ybase = reinterpret_cast<uint16_t*>(dw_hi ? A.yh : A.yl) + ((size_t)n * Cd + dc) * dHd * dWd + 8 * gimg;
 
     for (int c = c0; c <= c1; ++c) {
@@ -571,28 +642,29 @@ il_stream_kernel(const __grid_constant__ IlsArgs A, const __grid_constant__ CUte
       // ---- 5. depthwise tail over the chunk's rows --------------------------------------------------------
       if (dw_live) {
         const uint32_t t1b = (dw_hi ? xh : T1L) + dw_off;
-        for (int rr = 0; rr < dw_rows; ++rr) {
-          const int r = dw_rows * c + rr;                                // T1 row arriving; T2 row r-1; output row r-2
-          const uint32_t p = t1b + (uint32_t)rr * dw_rowstep;
-          uint32_t n1[6];
-          const uint4 m = lds128(p);
-          n1[0] = lds32(edgeL ? ZERO : p - (uint32_t)Sd * 16u + 12u);
-          n1[1] = m.x; n1[2] = m.y; n1[3] = m.z; n1[4] = m.w;
-          n1[5] = lds32(edgeR ? ZERO : p + (uint32_t)Sd * 16u);
-          const int tr = r - 1, orow = r - 2;
+        // T1 row r arriving; T2 row r-1; output row r-2.  Rows come in pairs (dw_rows is 4 or 2): the open rows swap roles
+        auto row = [&](float (&a2)[kIlsT2], float (&b2)[kIlsT2], float (&ao)[kIlsTO], float (&bo)[kIlsTO], int rr) {
+          const int r = dw_rows * c + rr, tr = r - 1, orow = r - 2;
           const bool make_t2 = tr >= 0 && tr >= out_lo - 1 && tr <= out_hi;
           const bool make_out = orow >= out_lo && orow < out_hi;
-          ils_dw_push<T>(t1w, t2w, n1, w1, b1, s1, w2, b2, s2, make_t2, mL, mR, make_out, ybase + (size_t)orow * dWd);
+          const uint32_t p = t1b + (uint32_t)rr * dw_rowstep;
+          float x[kIlsTX];
+          ils_dw_load<T>(x, p, hasB ? p + sd : ZERO, zeroL ? ZERO : p - sd + 12u, zeroR ? ZERO : p + 2u * sd);
+          ils_dw_push<T>(a2, b2, ao, bo, x, prm, make_t2, edg, make_out, ybase + (size_t)orow * dWd);
+        };
+        for (int rr = 0; rr < dw_rows; rr += 2) {
+          row(tl.s2a, tl.s2b, tl.soa, tl.sob, rr);
+          row(tl.s2b, tl.s2a, tl.sob, tl.soa, rr + 1);
         }
       }
     }
     // ---- image bottom: two rows of zero padding flush the last two output rows ----------------------------
     if (cb == cpi && dw_live) {
-      const uint32_t z[6] = {0u, 0u, 0u, 0u, 0u, 0u};
-      for (int rr = 0; rr < 2; ++rr) {
-        const int r = dHd + rr, tr = r - 1, orow = r - 2;
-        ils_dw_push<T>(t1w, t2w, z, w1, b1, s1, w2, b2, s2, tr < dHd, mL, mR, orow >= out_lo, ybase + (size_t)orow * dWd);
-      }
+      float z[kIlsTX];
+#pragma unroll
+      for (int i = 0; i < kIlsTX; ++i) z[i] = 0.f;
+      ils_dw_push<T>(tl.s2a, tl.s2b, tl.soa, tl.sob, z, prm, true, edg, dHd - 2 >= out_lo, ybase + (size_t)(dHd - 2) * dWd);
+      ils_dw_push<T>(tl.s2b, tl.s2a, tl.sob, tl.soa, z, prm, false, edg, dHd - 1 >= out_lo, ybase + (size_t)(dHd - 1) * dWd);
     }
     __syncthreads();          // every shared-memory read of this piece is done before the next piece's loads overwrite it
   }

@@ -522,7 +522,6 @@ bool plan_ils(const csnet_plan& P, const csnet_op_desc& op, const csnet::IlArgs&
   A.cpi = A.H / 4;
   auto r128 = [](int v) { return (v + 127) / 128 * 128; };
   bool found = false;
-  double best_cost = 0;
   csnet::IlsArgs best{};
   for (int ns = 1; ns <= 16; ++ns) {
     if (P.ils_force_ns > 0 && ns != P.ils_force_ns) continue;
@@ -530,7 +529,8 @@ bool plan_ils(const csnet_plan& P, const csnet_op_desc& op, const csnet::IlArgs&
     csnet::IlsArgs T = A;
     T.ns = ns; T.gsn = A.GH / ns; T.hl = ns > 1 ? 1 : 0;
     T.GR = T.gsn + 2 * T.hl; T.GLR = T.gsn / 2 + 2 * T.hl;
-    T.dw_warps = (T.Cho * T.gsn + T.Clo * (T.gsn / 2) + 31) / 32;        // tail tasks are packed: hi (channel, column)s, then lo ones
+    // tail tasks (a channel, two 8-pixel groups of a strip row) are packed: hi ones, then lo ones
+    T.dw_warps = (T.Cho * (T.gsn / 2) + T.Clo * ((T.gsn / 2 + 1) / 2) + 31) / 32;
     if (T.dw_warps < 4) T.dw_warps = 4;                                   // the GEMM needs one warpgroup
     const int warps = T.dw_warps;
     if (warps * 32 > csnet::kIlsMaxThreads || T.SH > 256 || T.SL > 256 || T.GR > 256) continue;
@@ -547,7 +547,8 @@ bool plan_ils(const csnet_plan& P, const csnet_op_desc& op, const csnet::IlArgs&
     T.off_bar = T.off_wbl + r128(T.NL * T.K16 * 2);
     T.off_zero = T.off_bar + 256;
     T.off_epi = T.off_zero + 128;                          // 4 tables of 64 floats + 512 bytes of scratch rows
-    T.off_xlo = T.off_epi + 1536;                          // stem: GEMM operand of the lo chunk (the ring holds image blocks)
+    T.off_dwp = T.off_epi + 1536;                          // depthwise-tail parameter records, one per hi / lo channel
+    T.off_xlo = T.off_dwp + r128((T.Cho + T.Clo) * csnet::kIlsDwpBytes);   // stem: GEMM operand of the lo chunk (the ring holds image blocks)
     int end = T.off_xlo + (stem ? r128(2 * T.GLR * T.SL * 16) : 0);
     // the last GEMM block of a chunk reads (never uses) up to 7 pixel groups past the chunk: keep them inside
     const int over_h = T.off_xh + T.hi_stage_bytes + nbh * 8 * T.SH * 16,
@@ -556,9 +557,11 @@ bool plan_ils(const csnet_plan& P, const csnet_op_desc& op, const csnet::IlArgs&
     end = over_l > end ? over_l : end;
     T.smem_bytes = end + 128;
     if (T.smem_bytes > 227 * 1024) continue;
-    // cost model: the depthwise tail (~55 % of a chunk) does not see the halo groups, everything else scales with them.
-    const double cost = 0.55 + 0.45 * T.GR / T.gsn;
-    if (!found || cost < best_cost) { best = T; best_cost = cost; found = true; }
+    // the depthwise tail's work does not depend on the strips, everything else scales with the tile's groups per strip
+    // group, GR / gsn = 1 + 2 hl / gsn, which only grows with ns: the first split that fits is the cheapest
+    best = T;
+    found = true;
+    break;
   }
   if (!found) return false;
   best.wh = il.wh; best.wl = il.wl;
