@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define CSNET_ABI_VERSION 6
+#define CSNET_ABI_VERSION 7
 
 enum { CSNET_F32 = 0, CSNET_F16 = 1, CSNET_BF16 = 2 };
 
@@ -238,6 +238,31 @@ int csnet_resize_logits_to_u8(const float* logits, int32_t N, int32_t H, int32_t
  */
 int csnet_plan_run_host_images_u8(csnet_plan* plan, int32_t N, const uint8_t* x_packed, int64_t x_bytes, const csnet_image_geom* geom,
                                   uint8_t* y_packed, int64_t y_bytes, const float* mean, const float* std, void* stream);
+
+/*
+ * Training data on the device (CSNet_training/utils/prepare_data.py:109-139 SalData.__getitem__, train.py:250-293 val).  A dataset
+ * is packed once: image i is uint8 [h][w][3] at byte src_off of x_packed, its mask uint8 [h][w] at byte dst_off of m_packed
+ * (csnet_image_geom as above).  Geometry and samples live on the DEVICE and are not checked there; the caller guarantees every
+ * index, window and offset.  Bad scalar arguments return CSNET_E_INVALID.  Asynchronous on `stream` (current device).
+ */
+typedef struct {
+  int32_t image;          /* index into geom */
+  int32_t y0, x0, h, w;   /* crop window img[y0:y0+h, x0:x0+w] */
+  int32_t flip;           /* 0 none, 1 'lr' (np.fliplr), 2 'ud' (np.flipud), applied after the crop */
+} csnet_train_sample;     /* 24 bytes */
+
+/* N training samples: x_nchw fp32 [N,3,H,W] = ((resize(crop/flip(x / 255)) - mean[c]) / std[c]) and target fp32 [N,1,H,W] =
+ * resize(crop/flip(m / 255)), evaluated in float64 and rounded once, the resize being csnet_resize_u8_to_input's.  mean / std are
+ * host float[3]; samples DEVICE [N]. */
+int csnet_train_batch_u8(const uint8_t* x_packed, const uint8_t* m_packed, const csnet_image_geom* geom, const csnet_train_sample* samples,
+                         int32_t N, int32_t H, int32_t W, const float* mean, const float* std, float* x_nchw, float* target, void* stream);
+
+/* Validation MAE per image (train.py:262-279): logits fp32 [N,1,H,W], image n's GT uint8 [h][w] at m_packed + geom[n].dst_off
+ * (geom DEVICE [N]).  mae DEVICE float64 [N] = mean |(int)(interp(sigmoid(z)) * 255) / 255 - g / 255|, interp being
+ * F.interpolate(size=(h, w), mode='bilinear', align_corners=False) in fp32.  Deterministic: no atomics, the same bits for an image
+ * in any batch. */
+int csnet_val_mae_u8(const float* logits, int32_t N, int32_t H, int32_t W, const uint8_t* m_packed, const csnet_image_geom* geom,
+                     double* mae, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Training primitives (fp32 planar NCHW device tensors).  The reference trains through torch autograd

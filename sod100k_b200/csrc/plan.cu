@@ -1337,6 +1337,27 @@ int csnet_resize_logits_to_u8(const float* logits, int32_t N, int32_t H, int32_t
   return CSNET_OK;
 }
 
+int csnet_train_batch_u8(const uint8_t* x_packed, const uint8_t* m_packed, const csnet_image_geom* geom, const csnet_train_sample* samples,
+                         int32_t N, int32_t H, int32_t W, const float* mean, const float* stdv, float* x_nchw, float* target, void* stream) {
+  if (!x_packed || !m_packed || !geom || !samples || !mean || !stdv || !x_nchw || !target)
+    return fail(CSNET_E_INVALID, "csnet_train_batch_u8: null argument");
+  if (N <= 0 || N > 65535 || H <= 0 || W <= 0 || H > csnet::kMaxImageSide || W > csnet::kMaxImageSide)
+    return fail(CSNET_E_INVALID, "csnet_train_batch_u8: N outside [1, 65535] or H, W outside [1, 32767]");
+  csnet::launch_train_batch(x_packed, m_packed, geom, samples, N, H, W, csnet::img_norm(mean, stdv), x_nchw, target, (cudaStream_t)stream);
+  CU_CHECK(cudaGetLastError());
+  return CSNET_OK;
+}
+
+int csnet_val_mae_u8(const float* logits, int32_t N, int32_t H, int32_t W, const uint8_t* m_packed, const csnet_image_geom* geom,
+                     double* mae, void* stream) {
+  if (!logits || !m_packed || !geom || !mae) return fail(CSNET_E_INVALID, "csnet_val_mae_u8: null argument");
+  if (N <= 0 || N > 65535 || H <= 0 || W <= 0 || H > csnet::kMaxImageSide || W > csnet::kMaxImageSide)
+    return fail(CSNET_E_INVALID, "csnet_val_mae_u8: N outside [1, 65535] or H, W outside [1, 32767]");
+  csnet::launch_val_mae(logits, N, H, W, m_packed, geom, mae, (cudaStream_t)stream);
+  CU_CHECK(cudaGetLastError());
+  return CSNET_OK;
+}
+
 // csnet_plan_run_host_images_u8's geometry, checked before anything is copied or launched.
 static int check_images(const csnet_image_geom* g, int32_t N, int64_t x_bytes, int64_t y_bytes) {
   for (int32_t i = 0; i < N; ++i) {

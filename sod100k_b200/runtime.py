@@ -13,7 +13,7 @@ from . import ir
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libcsnet_b200.so")
-ABI_VERSION = 6
+ABI_VERSION = 7
 PARAM_EPOCH = 0      # bumped by in-place parameter updates that bypass torch's version counters (FusedAdam)
 _lib = None
 
@@ -22,7 +22,7 @@ SYMBOLS = ("csnet_abi_version", "csnet_last_error", "csnet_device_count", "csnet
            "csnet_plan_set_blob", "csnet_plan_run", "csnet_plan_profile", "csnet_plan_tensor_ptr", "csnet_plan_read_tensor", "csnet_plan_op_kernel", "csnet_plan_launches",
            "csnet_plan_arena_bytes", "csnet_plan_destroy", "csnet_plan_run_host", "csnet_plan_run_host_u8",
            "csnet_resize_u8_to_input", "csnet_resize_logits_to_u8", "csnet_plan_run_host_images_u8",
-           "csnet_train_last_error", "csnet_train_bn_stats", "csnet_train_bn_prelu_fwd", "csnet_train_bn_prelu_bwd",
+           "csnet_train_batch_u8", "csnet_val_mae_u8", "csnet_train_last_error", "csnet_train_bn_stats", "csnet_train_bn_prelu_fwd", "csnet_train_bn_prelu_bwd",
            "csnet_train_dw_conv", "csnet_train_dw_wgrad", "csnet_train_dw_bwd", "csnet_train_mix_fwd", "csnet_train_mix_dgrad",
            "csnet_train_mix_wgrad", "csnet_train_pool_fwd", "csnet_train_pool_bwd", "csnet_slim_gather", "csnet_train_bce", "csnet_train_adam", "csnet_salmetric_hist")
 
@@ -39,6 +39,15 @@ class ImageGeom(C.Structure):
 
 assert C.sizeof(ImageGeom) == 24
 GEOM_DTYPE = np.dtype(ImageGeom)
+
+
+class TrainSample(C.Structure):
+    """csnet_train_sample: crop image `image` of the packed set to [y0:y0+h, x0:x0+w], then flip it (0 none, 1 'lr', 2 'ud')."""
+    _fields_ = [("image", C.c_int32), ("y0", C.c_int32), ("x0", C.c_int32), ("h", C.c_int32), ("w", C.c_int32), ("flip", C.c_int32)]
+
+
+assert C.sizeof(TrainSample) == 24
+SAMPLE_DTYPE = np.dtype(TrainSample)
 
 
 def image_geometry(sizes) -> np.ndarray:
@@ -99,6 +108,11 @@ def load_library(path: Optional[str] = None):
     lib.csnet_plan_run_host_images_u8.restype = C.c_int
     lib.csnet_plan_run_host_images_u8.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
                                                   C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_void_p]
+    lib.csnet_train_batch_u8.restype = C.c_int
+    lib.csnet_train_batch_u8.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                         C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.csnet_val_mae_u8.restype = C.c_int
+    lib.csnet_val_mae_u8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.csnet_slim_gather.restype = C.c_int
     lib.csnet_slim_gather.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     lib.csnet_train_last_error.restype = C.c_char_p
@@ -127,6 +141,22 @@ def resize_logits_to_u8(logits_ptr: int, N: int, H: int, W: int, geom_dev_ptr: i
     lib = load_library()
     _check(lib, lib.csnet_resize_logits_to_u8(logits_ptr, int(N), int(H), int(W), geom_dev_ptr, y_packed_ptr, stream),
            "csnet_resize_logits_to_u8")
+
+
+def train_batch_u8(x_packed_ptr: int, m_packed_ptr: int, geom_dev_ptr: int, samples_dev_ptr: int, N: int, H: int, W: int, mean, std,
+                   x_nchw_ptr: int, target_ptr: int, stream: int = 0):
+    """Device to device: packed uint8 images and masks, a crop / flip per sample -> fp32 input [N,3,H,W] and target [N,1,H,W]
+    (csnet_train_batch_u8)."""
+    lib = load_library()
+    m, s_ = (C.c_float * 3)(*mean), (C.c_float * 3)(*std)
+    _check(lib, lib.csnet_train_batch_u8(x_packed_ptr, m_packed_ptr, geom_dev_ptr, samples_dev_ptr, int(N), int(H), int(W), m, s_,
+                                         x_nchw_ptr, target_ptr, stream), "csnet_train_batch_u8")
+
+
+def val_mae_u8(logits_ptr: int, N: int, H: int, W: int, m_packed_ptr: int, geom_dev_ptr: int, mae_ptr: int, stream: int = 0):
+    """Device to device: fp32 logits [N,1,H,W] and each image's uint8 GT -> float64 MAE [N] (csnet_val_mae_u8)."""
+    lib = load_library()
+    _check(lib, lib.csnet_val_mae_u8(logits_ptr, int(N), int(H), int(W), m_packed_ptr, geom_dev_ptr, mae_ptr, stream), "csnet_val_mae_u8")
 
 
 class Plan:
