@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define CSNET_ABI_VERSION 7
+#define CSNET_ABI_VERSION 8
 
 enum { CSNET_F32 = 0, CSNET_F16 = 1, CSNET_BF16 = 2 };
 
@@ -228,6 +228,15 @@ int csnet_resize_u8_to_input(const uint8_t* x_packed, const csnet_image_geom* ge
  * DEVICE; the maps must not overlap). */
 int csnet_resize_logits_to_u8(const float* logits, int32_t N, int32_t H, int32_t W, const csnet_image_geom* geom, uint8_t* y_packed,
                               void* stream);
+
+/* SalMetric on the maps csnet_resize_logits_to_u8 would write, without the png round trip (CSNet/eval.py, sal_metric.cpp:86-120).
+ * Device to device, asynchronous on `stream` (current device): logits fp32 [N,1,H,W], geometry on the DEVICE, image n's GT uint8 [h][w]
+ * at m_packed + dst_off (the masks of a SalImages set).  Each map byte q is computed as csnet_resize_logits_to_u8 computes it; per
+ * image n: hist_all[n][q]++, hist_pos[n][q]++ where gt > 128, abs_sum[n] += |q - gt| (DEVICE uint32 [N][256], [N][256], uint64 [N],
+ * zeroed by the call).  The counts are exact and the same for an image in any batch.  y_packed may be NULL: with it the maps are
+ * also stored at y_packed + dst_off, without it no map is written. */
+int csnet_salmetric_images_u8(const float* logits, int32_t N, int32_t H, int32_t W, const csnet_image_geom* geom, const uint8_t* m_packed,
+                              uint8_t* y_packed, uint32_t* hist_all, uint32_t* hist_pos, unsigned long long* abs_sum, void* stream);
 
 /*
  * Host to host, synchronised like csnet_plan_run_host: x_packed (x_bytes bytes) and the HOST geometry geom[N] in, the maps out to

@@ -11,6 +11,7 @@
 //        returns float32), s * 255.f truncated to uint8
 // Where the coordinate lands on a sample (t == 0, every pixel at identity size) the lerps return that sample exactly, so a batch
 // already at the network size gives the bytes of csnet_plan_run_host_u8.
+//   eval: the `out` bytes counted against each image's GT into SalMetric's histograms (sal_metric.cpp:86-120), the map optional
 //
 // Training (CSNet_training/utils/prepare_data.py:109-139, train.py:250-293) reuses the same resize:
 //   train: a crop window and a flip per sample remap the taps of the cropped, flipped array into the stored image; image as `in`,
@@ -178,6 +179,49 @@ __global__ void __launch_bounds__(kImgThreads) resize_out_u8_kernel(const float*
   }
 }
 
+// SalMetric counts (sal_metric.cpp:86-120) of each image's map as resize_out_u8_kernel computes it, against the image's uint8 GT
+// [h][w] at m + dst_off; the map is stored at y + dst_off only when y is non-null.  Grid as resize_out_u8_kernel.  Each warp counts
+// into its own shared histograms (a saliency map piles most pixels into a few bins), the block adds them to image n's global ones
+// with integer atomics: the counts are exact and do not depend on the grid or the batch.  hist_all / hist_pos / abs_sum start at 0.
+__global__ void __launch_bounds__(kImgThreads) salmetric_images_u8_kernel(const float* __restrict__ z, int H, int W,
+                                                                         const csnet_image_geom* __restrict__ geom,
+                                                                         const uint8_t* __restrict__ m, uint8_t* __restrict__ y,
+                                                                         uint32_t* __restrict__ hist_all, uint32_t* __restrict__ hist_pos,
+                                                                         unsigned long long* __restrict__ abs_sum) {
+  constexpr int kWarps = kImgThreads / 32;
+  __shared__ uint32_t ha[kWarps][256], hp[kWarps][256];
+  __shared__ unsigned long long sd;
+  const int n = blockIdx.y;
+  const csnet_image_geom g = geom[n];
+  const int64_t hw = (int64_t)g.h * g.w;
+  if ((int64_t)blockIdx.x * kImgThreads >= hw) return;         // the whole block lies past a small image's end
+  for (int i = threadIdx.x; i < kWarps * 256; i += kImgThreads) { (&ha[0][0])[i] = 0u; (&hp[0][0])[i] = 0u; }
+  if (threadIdx.x == 0) sd = 0ull;
+  __syncthreads();
+  const float* zn = z + (int64_t)n * H * W;
+  const uint8_t* gt = m + g.dst_off;
+  uint32_t* wa = ha[threadIdx.x >> 5];
+  uint32_t* wp = hp[threadIdx.x >> 5];
+  unsigned long long d = 0;
+  for (int64_t p = (int64_t)blockIdx.x * kImgThreads + threadIdx.x; p < hw; p += (int64_t)gridDim.x * kImgThreads) {
+    const int oy = (int)p / g.w, ox = (int)p - oy * g.w;     // h * w < 2^31
+    const uint8_t q = img_out_value(zn, W, img_tap(oy, H, g.h), img_tap(ox, W, g.w));
+    if (y) y[g.dst_off + p] = q;
+    const int t = gt[p];
+    atomicAdd(&wa[q], 1u);
+    if (t > 128) atomicAdd(&wp[q], 1u);
+    d += (unsigned)(q > t ? q - t : t - q);
+  }
+  atomicAdd(&sd, d);
+  __syncthreads();
+  uint32_t sa = 0, sp = 0;                                      // kImgThreads == 256: one bin per thread
+#pragma unroll
+  for (int w = 0; w < kWarps; ++w) { sa += ha[w][threadIdx.x]; sp += hp[w][threadIdx.x]; }
+  if (sa) atomicAdd(hist_all + (int64_t)n * 256 + threadIdx.x, sa);
+  if (sp) atomicAdd(hist_pos + (int64_t)n * 256 + threadIdx.x, sp);
+  if (threadIdx.x == 0 && sd) atomicAdd(abs_sum + n, sd);
+}
+
 // Training batch from a packed uint8 dataset (SalData.__getitem__ in train mode, CSNet_training/utils/prepare_data.py:109-139):
 // sample n crops its image and mask to (h, w) at (y0, x0), flips them (1 'lr', 2 'ud') and resizes both to (H, W).  The crop and
 // flip only move the taps (img_tap_crop).  Grid and column taps as resize_in_u8_kernel; y fp32 [N,3,H,W], target fp32 [N,1,H,W].
@@ -264,6 +308,14 @@ inline void launch_resize_out(const float* z, int N, int H, int W, const csnet_i
                               cudaStream_t stream) {
   const int bx = (32 * num_sms + N - 1) / N;
   resize_out_u8_kernel<<<dim3((unsigned)bx, (unsigned)N), kImgThreads, 0, stream>>>(z, H, W, geom, y);
+}
+
+inline void launch_salmetric_images(const float* z, int N, int H, int W, const csnet_image_geom* geom, const uint8_t* m, uint8_t* y,
+                                    uint32_t* hist_all, uint32_t* hist_pos, unsigned long long* abs_sum, int num_sms, cudaStream_t stream) {
+  static_assert(kImgThreads == 256, "one histogram bin per thread");
+  const int bx = (32 * num_sms + N - 1) / N;
+  salmetric_images_u8_kernel<<<dim3((unsigned)bx, (unsigned)N), kImgThreads, 0, stream>>>(z, H, W, geom, m, y, hist_all, hist_pos,
+                                                                                          abs_sum);
 }
 
 inline void launch_train_batch(const uint8_t* x, const uint8_t* m, const csnet_image_geom* geom, const csnet_train_sample* samples, int N,

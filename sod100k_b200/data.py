@@ -10,6 +10,8 @@ draws them, cross PCIe.  The training loop of train.py becomes
     for idx in torch.randperm(len(ds)).split(batch_size):
         if len(idx) == batch_size:                                  # drop_last
             loss = trainer.step(*ds.train_batch(idx, rng))
+
+and a test set is scored like CSNet/test.py followed by eval.py with `SalImages(images, gts).evaluate(model)`.
 """
 from __future__ import annotations
 
@@ -170,3 +172,40 @@ class SalImages:
         g = self._upload(self.geom_host[idx])
         runtime.val_mae_u8(z.data_ptr(), N, H, W, self.m.data_ptr(), g.data_ptr(), mae.data_ptr(), self._stream())
         return mae
+
+    def evaluate(self, model, size=None, batch: int = 32, maps: bool = False, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+        """CSNet/test.py followed by eval.py (sal_metric.cpp) on this set, on the device from packed images to scores: each image goes
+        through `model`'s engine as ModelEngine.forward_images_u8(images, size, batch=batch) runs it (size=None: TEST.IMAGE_H = 0,
+        every image at its own size padded to multiples of 16), and its uint8 map at the image's original size is scored against its
+        mask by csnet_salmetric_images_u8.  Only the counts, 2 x 256 + 1 numbers per image, come to the host, where SalMetric.add_images
+        turns them into scores, adding the images in input order as sal_metric.cpp does.  Returns SalMetric.compute()'s dict (max_f,
+        mean_f, precision, recall, mean_precision, mean_recall, mae, argmax); with maps=True, (scores, maps) where maps are each
+        image's uint8 [h, w] map on the device, in input order."""
+        from .engine import image_runs
+        from .salmetric import SalMetric
+
+        eng = model.engine()
+        order, runs = image_runs(self.sizes, size, batch)
+        g = self._upload(self.geom_host[order])
+        N = len(self)
+        hist_all = torch.empty((N, 256), dtype=torch.int32, device=self.device)
+        hist_pos = torch.empty((N, 256), dtype=torch.int32, device=self.device)
+        abs_sum = torch.empty(N, dtype=torch.int64, device=self.device)
+        y = torch.empty(self.m.numel(), dtype=torch.uint8, device=self.device) if maps else None
+        stream = self._stream()
+
+        def score(logits, a, b, H, W, g_run):
+            runtime.salmetric_images_u8(logits.data_ptr(), b - a, H, W, g_run, self.m.data_ptr(), y.data_ptr() if maps else 0,
+                                        hist_all[a].data_ptr(), hist_pos[a].data_ptr(), abs_sum[a].data_ptr(), stream)
+
+        eng.run_packed_images(self.x, g, runs, size is None, mean, std, score)
+        inv = np.argsort(np.asarray(order, np.int64))
+        ha, hp, ad = (t.cpu().numpy()[inv] for t in (hist_all, hist_pos, abs_sum))
+        hw = self.sizes[:, 0] * self.sizes[:, 1]
+        metric = SalMetric()
+        metric.add_images(ha, hp, ad, hw)
+        scores = metric.compute()
+        if not maps:
+            return scores
+        offs = self.geom_host["dst_off"].tolist()
+        return scores, [y[o:o + int(n)].view(int(h), int(w)) for o, n, (h, w) in zip(offs, hw, self.sizes)]

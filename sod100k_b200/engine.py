@@ -3,7 +3,8 @@ when parameters change.  This is the host logic between the `nn.Module` surface 
 from __future__ import annotations
 
 import os
-from typing import Dict, Tuple
+from collections import OrderedDict
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -22,6 +23,39 @@ def _has_hooks(model) -> bool:
 
 
 _PROBES = {}
+
+NATIVE_PLAN_BUDGET = 2 << 30        # bytes of arena the native-size plans of one engine may keep resident between calls
+
+
+def native_size(h: int, w: int) -> Tuple[int, int]:
+    """The network input of an h x w image when CSNet/test.py runs with TEST.IMAGE_H = 0 (test.py:75-84): the image itself when h and
+    w are multiples of 16, else resized to (ceil(h / 16) * 16, ceil(w / 16) * 16)."""
+    if h % 16 or w % 16:
+        return (h + 15) // 16 * 16, (w + 15) // 16 * 16
+    return h, w
+
+
+def image_runs(sizes: Sequence, size: Optional[Tuple[int, int]], batch: Optional[int]):
+    """How forward_images_u8 and SalImages.evaluate cut a set of (h, w) images into network runs.  Returns (order, runs): `order` lists
+    the images in run order, and each run (a, b, H, W) takes order[a:b] at the network size H x W.  size=(H, W) keeps the input order
+    and runs everything at that size; size=None groups the images by native_size, in ascending padded size so that one pass meets each
+    size once.  No run holds more than `batch` images (None: no limit)."""
+    if batch is not None and int(batch) < 1:
+        raise ValueError(f"batch must be at least 1, got {batch}")
+    hw = [(int(h), int(w)) for h, w in sizes]
+    net = [native_size(h, w) for h, w in hw] if size is None else [(int(size[0]), int(size[1]))] * len(hw)
+    order = sorted(range(len(hw)), key=lambda i: net[i]) if size is None else list(range(len(hw)))
+    step = len(hw) if batch is None else int(batch)
+    runs: List[Tuple[int, int, int, int]] = []
+    a = 0
+    while a < len(order):
+        H, W = net[order[a]]
+        b = a
+        while b < len(order) and b - a < step and net[order[b]] == (H, W):
+            b += 1
+        runs.append((a, b, H, W))
+        a = b
+    return order, runs
 
 
 def param_version(tensors, epoch: int = 0, owner=None) -> int:
@@ -57,6 +91,8 @@ class ModelEngine:
         self.frozen = False
         self._epoch = 0
         self._pinned_images = None          # forward_images_u8's packed host input, reused across calls
+        self._native_plans: "OrderedDict[Tuple, runtime.Plan]" = OrderedDict()     # least recently used first
+        self.native_plan_budget = NATIVE_PLAN_BUDGET
 
     def set_precision(self, dtype: str):
         if dtype not in ir.DTYPE_NAMES:
@@ -78,8 +114,13 @@ class ModelEngine:
         return {k: v.detach().cpu() for k, v in self.model.state_dict().items()}
 
     def plan_for(self, N: int, H: int, W: int, device: torch.device) -> runtime.Plan:
-        key = (H, W, self.dtype, device.index or 0)
-        plan = self._plans.get(key)
+        return self._plan_in(self._plans, (H, W, self.dtype, device.index or 0), N)
+
+    def _plan_in(self, plans: Dict[Tuple, runtime.Plan], key: Tuple, N: int) -> runtime.Plan:
+        """The plan of `key` = (H, W, dtype, device, ...) in `plans` for a batch of N, created, refreshed after a parameter change,
+        or rebuilt when N outgrows it."""
+        H, W, dev = key[0], key[1], key[3]
+        plan = plans.get(key)
         if plan is not None and self.frozen and plan.max_batch >= N:
             return plan
         ver = self._version()
@@ -87,22 +128,44 @@ class ModelEngine:
             prog = compiler.compile_csnet(self.model.layer_config, self._state(), H, W, self.dtype)
             if plan is not None:
                 plan.close()
-            plan = runtime.Plan(prog, max_batch=N, device=key[3])
-            self._plans[key] = plan
+            plan = runtime.Plan(prog, max_batch=N, device=dev)
+            plans[key] = plan
         elif self._plan_version.get(key) != ver:
             prog = compiler.compile_csnet(self.model.layer_config, self._state(), H, W, self.dtype)
             if prog.signature() == plan.prog.signature():
-                plan.set_blob(prog.blob, torch.cuda.current_stream(device).cuda_stream)
+                plan.set_blob(prog.blob, torch.cuda.current_stream(dev).cuda_stream)
                 plan.prog = prog
             else:
                 # new weights changed the program itself (a 16-bit overflow veto, a fused block falling back, ...): the kernel
                 # choices frozen at plan creation no longer fit -> rebuild the plan
                 max_batch = plan.max_batch
                 plan.close()
-                plan = runtime.Plan(prog, max_batch=max_batch, device=key[3])
-                self._plans[key] = plan
+                plan = runtime.Plan(prog, max_batch=max_batch, device=dev)
+                plans[key] = plan
         self._plan_version[key] = ver
         return plan
+
+    def native_plan(self, N: int, H: int, W: int, device: torch.device) -> runtime.Plan:
+        """plan_for for the padded sizes of `forward_images_u8(size=None)`: these plans live in a cache of their own whose arenas
+        `trim_native_plans` keeps within `native_plan_budget` bytes, so a test set of many image sizes does not keep one arena per
+        size on the device.  The fixed-size plans of plan_for are not part of it."""
+        key = (H, W, self.dtype, device.index or 0, "native")
+        plan = self._plan_in(self._native_plans, key, N)
+        self._native_plans.move_to_end(key)
+        return plan
+
+    def trim_native_plans(self) -> None:
+        """Close native-size plans, least recently used first, until their arenas (csnet_plan_arena_bytes) fit the budget."""
+        total = sum(p.arena_bytes for p in self._native_plans.values())
+        if total <= self.native_plan_budget:
+            return
+        for dev in {k[3] for k in self._native_plans}:
+            torch.cuda.synchronize(dev)                  # work queued on a plan's arena or graphs ends before the plan goes
+        while self._native_plans and total > self.native_plan_budget:
+            key, plan = self._native_plans.popitem(last=False)
+            total -= plan.arena_bytes
+            self._plan_version.pop(key, None)
+            plan.close()
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if x.dim() != 4 or x.shape[1] != 3:
@@ -165,43 +228,76 @@ class ModelEngine:
             raise ValueError(f"image {i}: h and w must lie in [1, 32767], got {tuple(im.shape[:2])}")
         return im.contiguous()
 
-    def forward_images_u8(self, images, size=(224, 224), device: int = 0, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+    def forward_images_u8(self, images, size=(224, 224), device: int = 0, mean=IMAGENET_MEAN, std=IMAGENET_STD, batch: int = None):
         """CSNet/test.py:71-98 for a batch of images of any sizes, both skimage resizes included: each uint8 [h, w, 3] image is
-        resized to `size` (skimage >= 0.19 `resize(..., mode='reflect', anti_aliasing=False)`), normalised, run through the network,
-        and its sigmoid map resized back to (h, w) and quantised to uint8.  Returns the uint8 [h_i, w_i] maps in input order.
+        resized to its network size (skimage >= 0.19 `resize(..., mode='reflect', anti_aliasing=False)`), normalised, run through the
+        network, and its sigmoid map resized back to (h, w) and quantised to uint8.  Returns the uint8 [h_i, w_i] maps in input order.
+
+        size=(H, W) is test.py with TEST.IMAGE_H / IMAGE_W set: every image goes in at H x W.  size=None is TEST.IMAGE_H = 0: every
+        image goes in at its own size, resized to native_size(h, w) (the next multiples of 16) only when h or w is not a multiple of
+        16.  The images are then grouped by that size, one plan per size from a cache bounded by `native_plan_budget`.  No network
+        run takes more than `batch` images (None: all images of one size in one run).
 
         `images` are numpy arrays or CPU tensors (the host path: packed into a pinned buffer that is reused across calls, one
-        synchronised C call on plan `device`, the maps are views of one pinned buffer) or all CUDA tensors on one device (the
+        synchronised C call per run on plan `device`, the maps are views of one pinned buffer) or all CUDA tensors on one device (the
         device path: the resizes run around the network on the current stream, no host copies of pixels or maps)."""
         imgs = [self._image_u8(im, i) for i, im in enumerate(images)]
         if not imgs:
             return []
         if len({t.device for t in imgs}) > 1:
             raise ValueError("forward_images_u8 takes host images or CUDA images of one device, not a mix")
-        N, (H, W) = len(imgs), (int(size[0]), int(size[1]))
+        order, runs = image_runs([t.shape[:2] for t in imgs], size, batch)
+        imgs = [imgs[i] for i in order]
         geom = runtime.image_geometry([t.shape[:2] for t in imgs])
         hw = (geom["h"].astype(np.int64) * geom["w"]).tolist()
         total = sum(hw)
         if imgs[0].is_cuda:
             dev = imgs[0].device
-            plan = self.plan_for(N, H, W, dev)
-            stream = torch.cuda.current_stream(dev).cuda_stream
             x = torch.cat([t.reshape(-1) for t in imgs])
             g = torch.from_numpy(geom.view(np.uint8)).to(dev)
-            x_in = torch.empty((N, 3, H, W), dtype=torch.float32, device=dev)
-            runtime.resize_u8_to_input(x.data_ptr(), g.data_ptr(), N, H, W, mean, std, x_in.data_ptr(), stream)
-            logits = plan.forward(x_in)
             y = torch.empty(total, dtype=torch.uint8, device=dev)
-            runtime.resize_logits_to_u8(logits.data_ptr(), N, H, W, g.data_ptr(), y.data_ptr(), stream)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+
+            def store(logits, a, b, H, W, g_run):
+                runtime.resize_logits_to_u8(logits.data_ptr(), b - a, H, W, g_run, y.data_ptr(), stream)
+
+            self.run_packed_images(x, g, runs, size is None, mean, std, store)
         else:
             dev = torch.device("cuda", device)
-            plan = self.plan_for(N, H, W, dev)
             if self._pinned_images is None or self._pinned_images.numel() < 3 * total:
                 self._pinned_images = torch.empty(3 * total, dtype=torch.uint8, pin_memory=True)
             x = self._pinned_images[:3 * total]
             torch.cat([t.reshape(-1) for t in imgs], out=x)
             y = torch.empty(total, dtype=torch.uint8, pin_memory=True)
-            plan.run_host_images_u8(N, x.data_ptr(), 3 * total, geom, y.data_ptr(), total, mean, std,
-                                    torch.cuda.current_stream(dev).cuda_stream)
+            for k, (a, b, H, W) in enumerate(runs):
+                plan = self.native_plan(b - a, H, W, dev) if size is None else self.plan_for(b - a, H, W, dev)
+                g = geom[a:b].copy()
+                base, n_px = int(g["dst_off"][0]), sum(hw[a:b])
+                g["src_off"] -= 3 * base
+                g["dst_off"] -= base
+                plan.run_host_images_u8(b - a, x.data_ptr() + 3 * base, 3 * n_px, g, y.data_ptr() + base, n_px, mean, std,
+                                        torch.cuda.current_stream(dev).cuda_stream)
+                if size is None and (k + 1 == len(runs) or runs[k + 1][2:] != (H, W)):
+                    self.trim_native_plans()
         offs = geom["dst_off"].tolist()
-        return [y[o:o + n].view(t.shape[0], t.shape[1]) for o, n, t in zip(offs, hw, imgs)]
+        maps = [None] * len(imgs)
+        for i, o, n, t in zip(order, offs, hw, imgs):
+            maps[i] = y[o:o + n].view(t.shape[0], t.shape[1])
+        return maps
+
+    def run_packed_images(self, x_packed: torch.Tensor, geom_dev: torch.Tensor, runs, native: bool, mean, std, consume) -> None:
+        """The device side of forward_images_u8 for packed uint8 images on one device: for each run (a, b, H, W) of image_runs, entries
+        a..b-1 of the device geometry table `geom_dev` are resized to H x W (csnet_resize_u8_to_input) and run through the plan of
+        that size (native_plan when `native`, else plan_for), then consume(logits, a, b, H, W, geometry address of entry a) takes the
+        logits, on the current stream.  Native-size plans are trimmed to the budget after each size."""
+        dev = x_packed.device
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        for k, (a, b, H, W) in enumerate(runs):
+            n = b - a
+            plan = self.native_plan(n, H, W, dev) if native else self.plan_for(n, H, W, dev)
+            g = geom_dev.data_ptr() + a * runtime.GEOM_DTYPE.itemsize
+            x_in = torch.empty((n, 3, H, W), dtype=torch.float32, device=dev)
+            runtime.resize_u8_to_input(x_packed.data_ptr(), g, n, H, W, mean, std, x_in.data_ptr(), stream)
+            consume(plan.forward(x_in), a, b, H, W, g)
+            if native and (k + 1 == len(runs) or runs[k + 1][2:] != (H, W)):
+                self.trim_native_plans()

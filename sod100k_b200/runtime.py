@@ -13,7 +13,7 @@ from . import ir
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libcsnet_b200.so")
-ABI_VERSION = 7
+ABI_VERSION = 8
 PARAM_EPOCH = 0      # bumped by in-place parameter updates that bypass torch's version counters (FusedAdam)
 _lib = None
 
@@ -21,7 +21,7 @@ _lib = None
 SYMBOLS = ("csnet_abi_version", "csnet_last_error", "csnet_device_count", "csnet_plan_create",
            "csnet_plan_set_blob", "csnet_plan_run", "csnet_plan_profile", "csnet_plan_tensor_ptr", "csnet_plan_read_tensor", "csnet_plan_op_kernel", "csnet_plan_launches",
            "csnet_plan_arena_bytes", "csnet_plan_destroy", "csnet_plan_run_host", "csnet_plan_run_host_u8",
-           "csnet_resize_u8_to_input", "csnet_resize_logits_to_u8", "csnet_plan_run_host_images_u8",
+           "csnet_resize_u8_to_input", "csnet_resize_logits_to_u8", "csnet_salmetric_images_u8", "csnet_plan_run_host_images_u8",
            "csnet_train_batch_u8", "csnet_val_mae_u8", "csnet_train_last_error", "csnet_train_bn_stats", "csnet_train_bn_prelu_fwd", "csnet_train_bn_prelu_bwd",
            "csnet_train_dw_conv", "csnet_train_dw_wgrad", "csnet_train_dw_bwd", "csnet_train_mix_fwd", "csnet_train_mix_dgrad",
            "csnet_train_mix_wgrad", "csnet_train_pool_fwd", "csnet_train_pool_bwd", "csnet_slim_gather", "csnet_train_bce", "csnet_train_adam", "csnet_salmetric_hist")
@@ -105,6 +105,9 @@ def load_library(path: Optional[str] = None):
                                              C.POINTER(C.c_float), C.c_void_p, C.c_void_p]
     lib.csnet_resize_logits_to_u8.restype = C.c_int
     lib.csnet_resize_logits_to_u8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.csnet_salmetric_images_u8.restype = C.c_int
+    lib.csnet_salmetric_images_u8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_void_p]
     lib.csnet_plan_run_host_images_u8.restype = C.c_int
     lib.csnet_plan_run_host_images_u8.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
                                                   C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_void_p]
@@ -141,6 +144,15 @@ def resize_logits_to_u8(logits_ptr: int, N: int, H: int, W: int, geom_dev_ptr: i
     lib = load_library()
     _check(lib, lib.csnet_resize_logits_to_u8(logits_ptr, int(N), int(H), int(W), geom_dev_ptr, y_packed_ptr, stream),
            "csnet_resize_logits_to_u8")
+
+
+def salmetric_images_u8(logits_ptr: int, N: int, H: int, W: int, geom_dev_ptr: int, m_packed_ptr: int, y_packed_ptr: int,
+                        hist_all_ptr: int, hist_pos_ptr: int, abs_sum_ptr: int, stream: int = 0):
+    """Device to device: fp32 logits [N,1,H,W] and each image's uint8 GT -> SalMetric counts of the maps resize_logits_to_u8 would
+    write (uint32 [N,256] twice, uint64 [N]); the maps too when y_packed_ptr is non-zero (csnet_salmetric_images_u8)."""
+    lib = load_library()
+    _check(lib, lib.csnet_salmetric_images_u8(logits_ptr, int(N), int(H), int(W), geom_dev_ptr, m_packed_ptr, y_packed_ptr or None,
+                                              hist_all_ptr, hist_pos_ptr, abs_sum_ptr, stream), "csnet_salmetric_images_u8")
 
 
 def train_batch_u8(x_packed_ptr: int, m_packed_ptr: int, geom_dev_ptr: int, samples_dev_ptr: int, N: int, H: int, W: int, mean, std,

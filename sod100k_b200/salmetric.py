@@ -31,6 +31,20 @@ def _lib():
     return lib
 
 
+def image_scores(hist_all: np.ndarray, hist_pos: np.ndarray, abs_sum: np.ndarray, hw):
+    """Per image, from the device counts (host arrays hist_all / hist_pos [n, 256], abs_sum [n] as csnet_salmetric_hist and
+    csnet_salmetric_images_u8 produce them; hw the pixels per image, one number or [n]): precision and recall [n, 256] in float32
+    (sal_metric.cpp:99-120) and the MAE [n] in float64 (:86-97)."""
+    ha = np.asarray(hist_all).astype(np.int64)
+    hp = np.asarray(hist_pos).astype(np.int64)
+    # a = sal > th: pixels strictly above th = suffix sum from th + 1
+    a_sum = (ha[:, ::-1].cumsum(1)[:, ::-1] - ha).astype(np.float32)
+    ab = (hp[:, ::-1].cumsum(1)[:, ::-1] - hp).astype(np.float32)
+    b_sum = hp.sum(1).astype(np.float32)[:, None]
+    mae = np.asarray(abs_sum).astype(np.float64) / (255.0 * np.asarray(hw))
+    return (ab + EPSILON) / (a_sum + EPSILON), (ab + EPSILON) / (b_sum + EPSILON), mae
+
+
 class SalMetric:
     """Streaming evaluator: `update(prob, gt)` per batch (CUDA tensors), `compute()` at the end."""
 
@@ -59,16 +73,20 @@ class SalMetric:
                                       torch.cuda.current_stream(p.device).cuda_stream)
         if rc != 0:
             raise runtime.EngineError(f"csnet_salmetric_hist failed ({rc}): {lib.csnet_train_last_error().decode()}")
-        ha = hist_all.cpu().numpy().astype(np.int64)
-        hp = hist_pos.cpu().numpy().astype(np.int64)
-        # a = sal > th: pixels strictly above th = suffix sum from th + 1
-        a_sum = (ha[:, ::-1].cumsum(1)[:, ::-1] - ha).astype(np.float32)
-        ab = (hp[:, ::-1].cumsum(1)[:, ::-1] - hp).astype(np.float32)
-        b_sum = hp.sum(1).astype(np.float32)[:, None]
-        self._prec += ((ab + EPSILON) / (a_sum + EPSILON)).sum(0)
-        self._rec += ((ab + EPSILON) / (b_sum + EPSILON)).sum(0)
-        self._mae += float((abs_sum.cpu().numpy().astype(np.float64) / (255.0 * hw)).sum())
+        prec, rec, mae = image_scores(hist_all.cpu().numpy(), hist_pos.cpu().numpy(), abs_sum.cpu().numpy(), hw)
+        self._prec += prec.sum(0)
+        self._rec += rec.sum(0)
+        self._mae += float(mae.sum())
         self._n += n
+
+    def add_images(self, hist_all: np.ndarray, hist_pos: np.ndarray, abs_sum: np.ndarray, hw) -> None:
+        """Add n images from their device counts (host arrays, see image_scores) one after another, as sal_metric.cpp adds them:
+        running float64 sums in image order, so the scores equal oracle/salmetric.py's on the same maps."""
+        prec, rec, mae = image_scores(hist_all, hist_pos, abs_sum, hw)
+        self._prec += np.cumsum(prec, 0, dtype=np.float64)[-1]
+        self._rec += np.cumsum(rec, 0, dtype=np.float64)[-1]
+        self._mae += float(np.cumsum(mae)[-1])
+        self._n += len(mae)
 
     def compute(self) -> dict:
         if self._n == 0:
