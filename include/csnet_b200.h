@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define CSNET_ABI_VERSION 8
+#define CSNET_ABI_VERSION 9
 
 enum { CSNET_F32 = 0, CSNET_F16 = 1, CSNET_BF16 = 2 };
 
@@ -103,11 +103,22 @@ enum {
                              the fp32 input image (cin <= 3) with ksize = 3, pad = 1, paths[1].pool = 2; both branches are
                              3x3 convs of it (lo: of its 2x2 max-pool).  WH / WL are then [ru16(C)][32] with column
                              k = ci*9 + ky*3 + kx; the kernel builds the im2col planes in shared memory. */
-  CSNET_OP_MIXPROJ = 5     /* a MIX op whose Cmid-channel result is never stored: a 1x1 projection to the single dst channel
+  CSNET_OP_MIXPROJ = 5,    /* a MIX op whose Cmid-channel result is never stored: a 1x1 projection to the single dst channel
                              runs in the epilogue, dst = proj_b + sum_c proj_w[c] * prelu(mix[c] + bias[c])  (CSNet.forward,
                              csnet.py:383-384: fuse1x1 -> cls_layer).  paths / bias_off / slope_off describe the Cmid-channel
                              MIX; ext_off[0] = proj_w offset (Cmid floats), ext_off[1] = proj_b offset or -1,
                              ext_off[2] = Cmid (<= 80).  Tensor-core kernel only: 16-bit sources, stride-1 conv paths. */
+  CSNET_OP_RESIZE = 6      /* bilinear resize to the destination's size, any ratio (F.interpolate(size=dst (H, W), mode='bilinear',
+                             align_corners=False): CSF+Res2Net/networks/gOctConv.py:99,102 and csf_res2net.py:258):
+                               dst[:, cout0 + c] = (accumulate ? dst[:, cout0 + c] : 0) + bilinear(src[:, c0 + c]),  c < cout.
+                             Per axis scale = (float)in / out, source index max(scale * (d + 0.5) - 0.5, 0), the upper tap clamped
+                             at the border; the four taps are combined in fp32 in ATen's order, an accumulate adds once in fp32
+                             and rounds once to dst's dtype.  Any sizes >= 1 on either side; src / dst fp32, fp16 or bf16 each.
+                             paths[0]: src, c0, cin, cout0, cout with cin == cout and ksize == 0; pre_avg, pool, dil, stride,
+                             pad and up are unused and must be 0 or 1, w_off -1.  n_paths == 1, src != dst, dst2 == -1,
+                             bias_off == slope_off == -1.  ext_off[0] = accumulate flag (0 or 1), ext_off[1..23] == -1.
+                             An accumulate reads its destination: a plan with exactly two externals runs small batches through
+                             staging buffers (csnet_plan_run) that do not hold external 1's old values. */
 };
 
 /*

@@ -22,6 +22,7 @@
 #include "mix_tc.cuh"
 #include "dw_fast.cuh"
 #include "image_io.cuh"
+#include "resize.cuh"
 
 namespace {
 
@@ -173,7 +174,7 @@ struct TcChoice {
 };
 
 // The kernel (family) launch_op() runs for an op, chosen once per op when the plan is created (choose_kernel).
-enum class Kern : uint8_t { Msd, MixStream, MixTc, Pool2, Upsample, Resample, MixGeneric, Gn, IlStream, IlBlock, DwFast, DwGeneric };
+enum class Kern : uint8_t { Msd, MixStream, MixTc, Pool2, Upsample, Resample, MixGeneric, Gn, IlStream, IlBlock, DwFast, DwGeneric, Resize };
 
 // Small batches of a two-external plan up to this size replay a captured graph (csnet_plan_run).
 constexpr int kGraphMaxN = 8;
@@ -270,9 +271,27 @@ int validate(const csnet_plan& P) {
       return fail(CSNET_E_INVALID, buf);
     };
     if (op.kind != CSNET_OP_MIX && op.kind != CSNET_OP_DW && op.kind != CSNET_OP_ILBLOCK && op.kind != CSNET_OP_GN &&
-        op.kind != CSNET_OP_MIXPROJ)
+        op.kind != CSNET_OP_MIXPROJ && op.kind != CSNET_OP_RESIZE)
       return bad("unknown kind");
     if (op.dst < 0 || op.dst >= nt) return bad("dst out of range");
+    if (op.kind == CSNET_OP_RESIZE) {
+      if (op.n_paths != 1) return bad("RESIZE takes one path");
+      if (op.dst2 != -1 || op.bias_off != -1 || op.slope_off != -1) return bad("RESIZE has no second destination, bias or slope");
+      if (op.ext_off[0] != 0 && op.ext_off[0] != 1) return bad("RESIZE accumulate flag (ext_off[0]) must be 0 or 1");
+      for (int e = 1; e < CSNET_MAX_EXT; ++e)
+        if (op.ext_off[e] != -1) return bad("RESIZE uses ext_off[0] only");
+      const csnet_path_desc& q = op.paths[0];
+      if (q.src < 0 || q.src >= nt) return bad("path src out of range");
+      if (q.src == op.dst) return bad("in-place op");
+      const csnet_tensor_desc &S = P.tensors[q.src], &D = P.tensors[op.dst];
+      if (q.ksize != 0 || q.cin != q.cout) return bad("RESIZE path: ksize 0, cin == cout");
+      if (q.c0 < 0 || q.cin <= 0 || q.c0 + q.cin > S.C) return bad("path input channel slice");
+      if (q.cout0 < 0 || q.cout0 + q.cout > D.C) return bad("path output channel slice");
+      for (int v : {q.pre_avg, q.pool, q.dil, q.stride, q.pad, q.up})
+        if (v != 0 && v != 1) return bad("RESIZE path: pre_avg, pool, dil, stride, pad and up must be 0 or 1");
+      if (q.w_off != -1) return bad("RESIZE path has no weights (w_off -1)");
+      continue;
+    }
     if (op.kind == CSNET_OP_GN) {
       if (op.n_paths != 1) return bad("GN takes one input");
       const int a = op.paths[0].src, groups = op.paths[0].up;
@@ -735,6 +754,7 @@ TcChoice choose_tc(const csnet_plan& P, const csnet_op_desc& op) {
 // every sub-batch of a plan runs the same kernels, bit for bit.
 Kern choose_kernel(const csnet_plan& P, const csnet_op_desc& op, const OpLaunch& R) {
   const csnet_tensor_desc& D = P.tensors[op.dst];
+  if (op.kind == CSNET_OP_RESIZE) return Kern::Resize;
   if (is_msd(P, op)) return Kern::Msd;
   if (R.ms.n_in > 0 && (int64_t)P.max_batch * (D.H / csnet::kMsRows) >= (int64_t)2 * P.num_sms) return Kern::MixStream;
   if ((op.kind == CSNET_OP_MIX || op.kind == CSNET_OP_MIXPROJ) && R.tc.mt > 0) return Kern::MixTc;
@@ -777,8 +797,9 @@ constexpr int kSmemOptIn = 227 * 1024;
 const char* const kKernNames[] = {
     "msd_kernel (ms_direct.cuh, FP32 pipe)", "mix_stream_kernel (TMA + wgmma)", "mix_tc_kernel (mma.sync)",
     "pool2 / upsample / resample kernels", "pool2 / upsample / resample kernels", "pool2 / upsample / resample kernels",
-    "mix_generic_kernel", "gn kernels", "il_stream_kernel (TMA + wgmma)", "il_block_kernel (mma.sync, tiled)", "dw kernels", "dw kernels"};
-static_assert(sizeof kKernNames / sizeof kKernNames[0] == (size_t)Kern::DwGeneric + 1, "one name per Kern");
+    "mix_generic_kernel", "gn kernels", "il_stream_kernel (TMA + wgmma)", "il_block_kernel (mma.sync, tiled)", "dw kernels", "dw kernels",
+    "resize_kernel"};
+static_assert(sizeof kKernNames / sizeof kKernNames[0] == (size_t)Kern::Resize + 1, "one name per Kern");
 
 // Plan op i: choose its kernel and fill its launch record (kernel, static arguments, packed-weight buffers), and let the
 // kernel use the shared memory it needs.
@@ -1137,6 +1158,20 @@ static int launch_op(csnet_plan* P, size_t i, int32_t N, const void* const* ext_
         dim3 grid((strips * D.W + kThreads - 1) / kThreads, D.C, N);
         dw_generic_kernel<<<grid, kThreads, 0, stream>>>(A);
       }
+      break;
+    }
+    case Kern::Resize: {
+      // bilinear resize at any ratio (resize.cuh)
+      const csnet_path_desc& q = op.paths[0];
+      const csnet_tensor_desc& S = P->tensors[q.src];
+      csnet::RzArgs A{};
+      A.src = P->tensor_ptr(q.src, N, ext_ptrs);
+      A.dst = P->tensor_ptr(op.dst, N, ext_ptrs);
+      A.Cs = S.C; A.Hs = S.H; A.Ws = S.W; A.c0 = q.c0;
+      A.Cd = D.C; A.Hd = D.H; A.Wd = D.W; A.cout0 = q.cout0;
+      A.C = q.cout; A.accumulate = (int)op.ext_off[0];
+      A.sy = csnet::resize_scale(S.H, D.H); A.sx = csnet::resize_scale(S.W, D.W);
+      csnet::launch_resize(A, S.dtype, D.dtype, N, stream);
       break;
     }
   }

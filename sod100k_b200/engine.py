@@ -82,6 +82,23 @@ def param_version(tensors, epoch: int = 0, owner=None) -> int:
     return h
 
 
+def trim_plans(plans: "OrderedDict[Tuple, runtime.Plan]", budget: int, versions: Dict[Tuple, int], keep: Optional[Tuple] = None) -> None:
+    """Close plans of an LRU cache (least recently used first; keys (H, W, dtype, device, ...)) until their arenas
+    (csnet_plan_arena_bytes) fit `budget` bytes, dropping their parameter versions too.  The plan of key `keep`, if given, stays."""
+    total = sum(p.arena_bytes for p in plans.values())
+    if total <= budget:
+        return
+    for dev in {k[3] for k in plans}:
+        torch.cuda.synchronize(dev)                      # work queued on a plan's arena or graphs ends before the plan goes
+    for key in [k for k in plans if k != keep]:
+        if total <= budget:
+            break
+        plan = plans.pop(key)
+        total -= plan.arena_bytes
+        versions.pop(key, None)
+        plan.close()
+
+
 class ModelEngine:
     def __init__(self, model):
         self.model = model
@@ -156,16 +173,7 @@ class ModelEngine:
 
     def trim_native_plans(self) -> None:
         """Close native-size plans, least recently used first, until their arenas (csnet_plan_arena_bytes) fit the budget."""
-        total = sum(p.arena_bytes for p in self._native_plans.values())
-        if total <= self.native_plan_budget:
-            return
-        for dev in {k[3] for k in self._native_plans}:
-            torch.cuda.synchronize(dev)                  # work queued on a plan's arena or graphs ends before the plan goes
-        while self._native_plans and total > self.native_plan_budget:
-            key, plan = self._native_plans.popitem(last=False)
-            total -= plan.arena_bytes
-            self._plan_version.pop(key, None)
-            plan.close()
+        trim_plans(self._native_plans, self.native_plan_budget, self._plan_version)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if x.dim() != 4 or x.shape[1] != 3:

@@ -12,7 +12,7 @@ DTYPE_BYTES = {F32: 4, F16: 2, BF16: 2}
 DTYPE_NAMES = {"fp32": F32, "float32": F32, "fp16": F16, "float16": F16, "half": F16, "bf16": BF16, "bfloat16": BF16}
 MAX_PATHS = 8
 MAX_EXT = 24
-OP_MIX, OP_DW, OP_ILBLOCK, OP_GN, OP_MIXPROJ = 1, 2, 3, 4, 5
+OP_MIX, OP_DW, OP_ILBLOCK, OP_GN, OP_MIXPROJ, OP_RESIZE = 1, 2, 3, 4, 5, 6
 
 
 class TensorDesc(C.Structure):

@@ -6,18 +6,22 @@ Split of the forward:
   * `base` (Res2Net-50 v1b 26w4s backbone, 11 of the 19 GMAC): ordinary torch modules — cuDNN LIBRARY calls, run under
     fp16 autocast when the plan is 16-bit.  Not the product; kept on the library as SURVEY.md §7 step 9 recommends until
     the CSF head meets its bar.
-  * CSF head (`fuse` -> `ms` -> `fuse1x1` -> `cls_layer` -> x4): parameter containers lowered by compiler_r.py to one
+  * CSF head (`fuse` -> `ms` -> `fuse1x1` -> `cls_layer` -> bilinear to the input size): parameter containers lowered by compiler_r.py to one
     fused-op program on libcsnet_b200.so (GroupNorm variant).  No torch fallback for the head.
 """
 from __future__ import annotations
 
 import math
+from collections import OrderedDict
 
 import torch
 import torch.nn as nn
 from torch.nn import init
 
 from .. import compiler_r, runtime, splits
+
+
+PLAN_BUDGET = 2 << 30        # bytes of arena the head plans of one CSFNet may keep resident between calls
 
 
 class Bottle2neck(nn.Module):
@@ -165,8 +169,9 @@ class CSFNet(nn.Module):
         self.fuse1x1 = gOctaveCBR(cout, cout, kernel_size=(1, 1), padding=0, alpha_in=compiler_r.FUSE_OUT_SPLIT, alpha_out=[1])
         self.cls_layer = nn.Conv2d(cout, num_classes, kernel_size=1)
         self.precision = "fp32"
-        self._plans = {}
+        self._plans = OrderedDict()              # (h, w, precision, device) -> head plan, least recently used first
         self._plan_version = {}
+        self.plan_budget = PLAN_BUDGET
 
     def set_precision(self, dtype: str):
         self.precision = dtype
@@ -174,7 +179,7 @@ class CSFNet(nn.Module):
 
     def __getstate__(self):                      # device plans (ctypes handles) never travel with a copy / pickle
         d = dict(self.__dict__)
-        d["_plans"], d["_plan_version"] = {}, {}
+        d["_plans"], d["_plan_version"] = OrderedDict(), {}
         return d
 
     def __deepcopy__(self, memo):
@@ -183,7 +188,9 @@ class CSFNet(nn.Module):
         new = self.__class__.__new__(self.__class__)
         memo[id(self)] = new
         for k, v in self.__dict__.items():
-            new.__dict__[k] = {} if k in ("_plans", "_plan_version") else copy.deepcopy(v, memo)
+            if k not in ("_plans", "_plan_version"):
+                new.__dict__[k] = copy.deepcopy(v, memo)
+        new._plans, new._plan_version = OrderedDict(), {}
         return new
 
     def head_state(self):
@@ -202,12 +209,14 @@ class CSFNet(nn.Module):
         if self.training or torch.is_grad_enabled():
             raise NotImplementedError("CSF+Res2Net runs inference only (config 5): call under model.eval() and torch.no_grad()")
         n, _, h, w = x.shape
+        # any (h, w): the head program resizes between the backbone's ceil(h / 2) stages as the reference does.  One plan per size
+        # lives in an LRU cache whose arenas `plan_budget` bounds (the plan in use stays even when it alone exceeds the budget)
         feats = self.backbone(x.float())
         key = (h, w, self.precision, x.device.index or 0)
         plan = self._plans.get(key)
         # the head plan folds the head's parameters at creation: re-fold when they change (load_state_dict, weights_init,
         # `.data` writes — same version stamp as the CSNet engine), so head and backbone never run on different weights
-        from ..engine import param_version
+        from ..engine import param_version, trim_plans
 
         ver = param_version([t for k, t in list(self.named_parameters()) + list(self.named_buffers()) if not k.startswith("base.")])
         if plan is None or plan.max_batch < n:
@@ -225,6 +234,8 @@ class CSFNet(nn.Module):
                 plan.close()
                 plan = self._plans[key] = runtime.Plan(prog, max_batch=mb, device=key[3])
         self._plan_version[key] = ver
+        self._plans.move_to_end(key)
+        trim_plans(self._plans, self.plan_budget, self._plan_version, keep=key)
         y = torch.empty((n, 1, h, w), dtype=torch.float32, device=x.device)
         plan.run(n, [f.data_ptr() for f in feats] + [y.data_ptr()], torch.cuda.current_stream(x.device).cuda_stream)
         return y
