@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define CSNET_ABI_VERSION 9
+#define CSNET_ABI_VERSION 10
 
 enum { CSNET_F32 = 0, CSNET_F16 = 1, CSNET_BF16 = 2 };
 
@@ -354,6 +354,57 @@ int csnet_train_bce(const float* logits, const float* target, float* dlogits, fl
  * {float* p; const float* g; float* m; float* v; int32 n; float weight_decay} (40 bytes each). */
 int csnet_train_adam(const void* chunk_table_device, int32_t n_chunks, float lr, float beta1, float beta2, float eps, int32_t step,
                      float grad_scale, void* stream);
+
+/* ---- CSF+Res2Net head training (fp32; sod100k_b200/modular_r.py wraps them) ---------------------------------------------------
+ * Convolutions as an fp32 FMA implicit GEMM (csrc/gemm_f32.cuh).  One segment is one stride-1 convolution of a channel slice of
+ * `src` with a weight slice: element (co, ci, ky, kx) of the weight is w[co * ldw + ci * ksize * ksize + ky * ksize + kx]
+ * (a slice [co0:, ci0:] of an OIHW parameter is w = param + (co0 * Cin + ci0) * k * k, ldw = Cin * k * k).  ksize is 1, or 3
+ * with dilation `dil` and zero padding `dil`; every tensor has the destination's H x W.  All segments of one call share ksize.
+ * Split-K partials go to the caller's workspace `ws` and are merged in split order: no floating-point atomics, the same bits on
+ * every run.  splits = 0 / tile = 0 let the library choose; tile 1 is the 64x64 block tile, 2 the 128x128 one. */
+typedef struct {
+  const float* src;       /* fp32 [N, C, H, W]: fwd / wgrad the conv's input, dgrad the gradient of the conv's output tensor */
+  const float* w;         /* weight slice (unused by wgrad, which writes the gradient at the same layout) */
+  int32_t C, c0, cin;     /* channels of src; the conv reads input channels [c0, c0 + cin) (dgrad: c0 unused) */
+  int32_t cout0, cout;    /* the conv's output channels [cout0, cout0 + cout): fwd writes them, dgrad / wgrad read their gradient */
+  int32_t ksize, dil, ldw;
+} csnet_conv_seg;         /* 48 bytes */
+
+enum { CSNET_CONV_FWD = 0, CSNET_CONV_DGRAD = 1, CSNET_CONV_WGRAD = 2 };
+
+/* The launch a conv call makes: splits, the longest chain of fp32 additions one output element passes through before the split
+ * merge (chain), and the workspace bytes it needs.  Arguments as the call's. */
+int csnet_train_conv_plan(int32_t form, int32_t N, int32_t H, int32_t W, const csnet_conv_seg* segs, int32_t n_segs, int32_t splits,
+                          int32_t tile, int32_t* splits_out, int32_t* chain_out, int64_t* ws_bytes);
+/* dst[:, cout0:cout0+cout] (+)= bias + sum over segments of conv(src[:, c0:c0+cin], w): segments share cout0 / cout (and cin may
+ * differ); dst is fp32 [N, C, H, W]; bias [cout] or NULL; accumulate adds the old value once. */
+int csnet_train_conv_fwd(float* dst, int32_t N, int32_t C, int32_t H, int32_t W, const csnet_conv_seg* segs, int32_t n_segs,
+                         const float* bias, int32_t accumulate, int32_t splits, int32_t tile, float* ws, int64_t ws_bytes, void* stream);
+/* Data gradient: dsrc[:, c0:c0+cin] (+)= sum over segments of the transposed conv of src_s[:, cout0_s:cout0_s+cout_s] (each
+ * segment's src is the gradient of an output the source fed); every segment has cin = the slice width; dsrc is [N, C, H, W]. */
+int csnet_train_conv_dgrad(float* dsrc, int32_t N, int32_t C, int32_t H, int32_t W, int32_t c0, int32_t cin, const csnet_conv_seg* segs,
+                           int32_t n_segs, int32_t accumulate, int32_t splits, int32_t tile, float* ws, int64_t ws_bytes, void* stream);
+/* Weight gradient of one segment: dw[co * ldw + ci * k * k + t] (+)= sum over images and pixels of ddst[n, cout0 + co] times the
+ * input tap t of src[n, c0 + ci]; ddst is fp32 [N, Cd, H, W]. */
+int csnet_train_conv_wgrad(const float* ddst, int32_t N, int32_t Cd, int32_t H, int32_t W, const csnet_conv_seg* seg, float* dw,
+                           int32_t accumulate, int32_t splits, int32_t tile, float* ws, int64_t ws_bytes, void* stream);
+/* Bias gradient: db[c] = sum over images and pixels of ddst[n, c0 + c], images in order. */
+int csnet_train_bias_grad(const float* ddst, int32_t N, int32_t C, int32_t HW, int32_t c0, int32_t cout, float* db, void* stream);
+/* F.group_norm(z, groups, eps) statistics per (image, group) over (C / groups) * HW values: mean and biased variance [N * groups]. */
+int csnet_train_gn_stats(const float* z, int32_t N, int32_t C, int32_t HW, int32_t groups, float* mean, float* var, void* stream);
+/* y = PReLU(gamma[c] * (z - mean) * rsqrt(var + eps) + beta[c], slope[c]) with the (image, group) statistics above. */
+int csnet_train_gn_prelu_fwd(const float* z, float* y, int32_t N, int32_t C, int32_t HW, int32_t groups, const float* mean,
+                             const float* var, const float* gamma, const float* beta, const float* slope, float eps, void* stream);
+/* Autograd of the above (statistics depend on z): dz, and dgamma / dbeta / dslope [C] summed over images in order.  ws: 3 N C floats. */
+int csnet_train_gn_prelu_bwd(const float* z, const float* dy, float* dz, int32_t N, int32_t C, int32_t HW, int32_t groups,
+                             const float* mean, const float* var, const float* gamma, const float* beta, const float* slope, float eps,
+                             float* dgamma, float* dbeta, float* dslope, float* ws, void* stream);
+/* dst (+)= F.interpolate(src, size=(Hd, Wd), mode='bilinear', align_corners=False), fp32 [N, C, Hs, Ws] -> [N, C, Hd, Wd]: the
+ * CSNET_OP_RESIZE kernel.  _bwd is its exact adjoint: dsrc = the transposed tap matrix applied to ddst, gathered per source pixel. */
+int csnet_train_resize_fwd(const float* src, int32_t N, int32_t C, int32_t Hs, int32_t Ws, float* dst, int32_t Hd, int32_t Wd,
+                           int32_t accumulate, void* stream);
+int csnet_train_resize_bwd(const float* ddst, int32_t N, int32_t C, int32_t Hd, int32_t Wd, float* dsrc, int32_t Hs, int32_t Ws,
+                           void* stream);
 
 /* ---- evaluation: the counting part of SalMetric on the device (CSNet_training/SalMetric/src/sal_metric.cpp:86-120) ----
  * prob: device float32 [N][HW] saliency in [0,1] (after sigmoid); gt: device uint8 [N][HW] ground truth.  Per image:

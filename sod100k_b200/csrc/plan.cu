@@ -23,6 +23,7 @@
 #include "dw_fast.cuh"
 #include "image_io.cuh"
 #include "resize.cuh"
+#include "resize_adj.cuh"
 
 namespace {
 
@@ -862,6 +863,10 @@ int plan_op(csnet_plan& P, size_t i) {
 
 }  // namespace
 
+namespace csnet {
+void train_set_error(const char* msg);     // train_ops.cu: the message csnet_train_last_error returns
+}
+
 extern "C" {
 
 int csnet_abi_version(void) { return CSNET_ABI_VERSION; }
@@ -1369,6 +1374,39 @@ int csnet_resize_logits_to_u8(const float* logits, int32_t N, int32_t H, int32_t
   CU_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   csnet::launch_resize_out(logits, N, H, W, geom, y_packed, sms, (cudaStream_t)stream);
   CU_CHECK(cudaGetLastError());
+  return CSNET_OK;
+}
+
+// Training pair of the RESIZE op (fp32): the forward is launch_resize itself, the backward its adjoint (resize_adj.cuh).
+int csnet_train_resize_fwd(const float* src, int32_t N, int32_t C, int32_t Hs, int32_t Ws, float* dst, int32_t Hd, int32_t Wd,
+                           int32_t accumulate, void* stream) {
+  if (!src || !dst || N < 1 || N > 65535 || C < 1 || C > 8 * 65535 || Hs < 1 || Ws < 1 || Hd < 1 || Wd < 1) {
+    csnet::train_set_error("csnet_train_resize_fwd: bad arguments");
+    return CSNET_E_INVALID;
+  }
+  csnet::RzArgs A{};
+  A.src = src; A.dst = dst;
+  A.Cs = C; A.Hs = Hs; A.Ws = Ws; A.c0 = 0;
+  A.Cd = C; A.Hd = Hd; A.Wd = Wd; A.cout0 = 0;
+  A.C = C; A.accumulate = accumulate != 0;
+  A.sy = csnet::resize_scale(Hs, Hd); A.sx = csnet::resize_scale(Ws, Wd);
+  csnet::launch_resize(A, CSNET_F32, CSNET_F32, N, (cudaStream_t)stream);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { csnet::train_set_error(cudaGetErrorString(e)); return CSNET_E_CUDA; }
+  return CSNET_OK;
+}
+
+int csnet_train_resize_bwd(const float* ddst, int32_t N, int32_t C, int32_t Hd, int32_t Wd, float* dsrc, int32_t Hs, int32_t Ws,
+                           void* stream) {
+  if (!ddst || !dsrc || N < 1 || N > 65535 || C < 1 || C > 65535 || Hs < 1 || Ws < 1 || Hd < 1 || Wd < 1 || (int64_t)Hs * Ws > (1 << 30)) {
+    csnet::train_set_error("csnet_train_resize_bwd: bad arguments");
+    return CSNET_E_INVALID;
+  }
+  const dim3 grid((unsigned)((Hs * Ws + csnet::kRzAdjThreads - 1) / csnet::kRzAdjThreads), (unsigned)C, (unsigned)N);
+  csnet::resize_bwd_kernel<<<grid, csnet::kRzAdjThreads, 0, (cudaStream_t)stream>>>(ddst, dsrc, C, Hs, Ws, Hd, Wd,
+                                                                                   csnet::resize_scale(Hs, Hd), csnet::resize_scale(Ws, Wd));
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { csnet::train_set_error(cudaGetErrorString(e)); return CSNET_E_CUDA; }
   return CSNET_OK;
 }
 

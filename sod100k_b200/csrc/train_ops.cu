@@ -401,6 +401,11 @@ __global__ void __launch_bounds__(kT) salmetric_hist_kernel(const float* __restr
 
 }  // namespace
 
+namespace csnet {
+// The other training sources (train_csf.cu, plan.cu's resize pair) report through csnet_train_last_error too.
+void train_set_error(const char* msg) { t_err = msg; }
+}  // namespace csnet
+
 extern "C" {
 
 const char* csnet_train_last_error(void) { return t_err.c_str(); }

@@ -8,6 +8,8 @@ Split of the forward:
     the CSF head meets its bar.
   * CSF head (`fuse` -> `ms` -> `fuse1x1` -> `cls_layer` -> bilinear to the input size): parameter containers lowered by compiler_r.py to one
     fused-op program on libcsnet_b200.so (GroupNorm variant).  No torch fallback for the head.
+  * Training: when autograd records, the backbone runs on torch autograd and the head on modular_r.py's autograd Functions over the
+    fp32 training kernels (csnet_train_conv_* / _gn_* / _resize_*), so solver.py's train loop runs unchanged.
 """
 from __future__ import annotations
 
@@ -206,8 +208,15 @@ class CSFNet(nn.Module):
     def forward(self, x):
         if not x.is_cuda:
             raise runtime.EngineError("CSFNet (CUDA engine) needs CUDA tensors; there is no CPU path")
-        if self.training or torch.is_grad_enabled():
-            raise NotImplementedError("CSF+Res2Net runs inference only (config 5): call under model.eval() and torch.no_grad()")
+        if torch.is_grad_enabled() and (x.requires_grad or any(q.requires_grad for q in self.parameters())):
+            # training (CSF+Res2Net/solver.py:train): the backbone on torch autograd (cuDNN, fp32), the head on our fp32 training kernels
+            # (modular_r), logits with a grad_fn at the input's size
+            from .. import modular_r
+
+            return modular_r.csf_head(self, self.base(x.float()), x.shape[2:])
+        if self.training:
+            raise NotImplementedError("CSF+Res2Net runs inference under model.eval() and torch.no_grad(), and trains with autograd "
+                                      "recording (grad enabled, parameters or input requiring grad)")
         n, _, h, w = x.shape
         # any (h, w): the head program resizes between the backbone's ceil(h / 2) stages as the reference does.  One plan per size
         # lives in an LRU cache whose arenas `plan_budget` bounds (the plan in use stays even when it alone exceeds the budget)
