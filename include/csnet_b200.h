@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define CSNET_ABI_VERSION 10
+#define CSNET_ABI_VERSION 11
 
 enum { CSNET_F32 = 0, CSNET_F16 = 1, CSNET_BF16 = 2 };
 
@@ -283,6 +283,26 @@ int csnet_train_batch_u8(const uint8_t* x_packed, const uint8_t* m_packed, const
  * in any batch. */
 int csnet_val_mae_u8(const float* logits, int32_t N, int32_t H, int32_t W, const uint8_t* m_packed, const csnet_image_geom* geom,
                      double* mae, void* stream);
+
+/*
+ * CSF+Res2Net's test path (CSF+Res2Net/solver.py:62-78 with dataset.py:83-96 load_image_test): every image runs at its own size, so
+ * a call takes N images that are all H x W (each geom entry's h, w equal H, W) and nothing is resized.  Packed sets, geometry on the
+ * DEVICE (not checked there), CSNET_E_INVALID for a null pointer or N outside [1, 65535] or H, W outside [1, 32767], asynchronous on
+ * `stream` (current device), as the calls above.
+ */
+/* x_nchw fp32 [N,3,H,W] from the uint8 HWC images at src_off, with numpy's three roundings:
+ * x = f32(f64(f32(f64(f32(u) / 255.f) - mean[c])) / std[c]).  mean / std are host double[3]. */
+int csnet_csf_input_u8(const uint8_t* x_packed, const csnet_image_geom* geom, int32_t N, int32_t H, int32_t W, const double* mean,
+                       const double* std, float* x_nchw, void* stream);
+
+/* Logits fp32 [N,1,H,W] -> each image's map at y_packed + dst_off, q = saturate(rint(255.f * sigmoid(z))) with round half to even
+ * (cv2.imwrite of solver.test's fp32 array) and sigmoid = 1.f / (1.f + expf(-z)) as torch's CUDA kernel computes it. */
+int csnet_csf_maps_u8(const float* logits, int32_t N, int32_t H, int32_t W, const csnet_image_geom* geom, uint8_t* y_packed, void* stream);
+
+/* csnet_salmetric_images_u8 for the maps csnet_csf_maps_u8 writes: the same outputs, zeroed by the call, exact and the same for an
+ * image in any batch; y_packed may be NULL. */
+int csnet_salmetric_csf_u8(const float* logits, int32_t N, int32_t H, int32_t W, const csnet_image_geom* geom, const uint8_t* m_packed,
+                           uint8_t* y_packed, uint32_t* hist_all, uint32_t* hist_pos, unsigned long long* abs_sum, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Training primitives (fp32 planar NCHW device tensors).  The reference trains through torch autograd

@@ -17,6 +17,11 @@
 //   train: a crop window and a flip per sample remap the taps of the cropped, flipped array into the stored image; image as `in`,
 //          mask m / 255 bilinear in double rounded once to fp32
 //   val:   the per-image MAE of train.py's loop, whose resize back to the GT's size is F.interpolate (ATen's fp32 bilinear), not skimage
+//
+// CSF+Res2Net's test (CSF+Res2Net/solver.py:62-78, dataset.py:83-96) runs each image at its own size, so neither side resizes:
+//   csf in:  img_csf_in_value, numpy's three fp32 roundings of load_image_test
+//   csf out: img_csf_out_value, cv2.imwrite of the fp32 array 255 * sigmoid: rounded half to even and saturated, not truncated
+// The map and SalMetric kernels are templates on the per-pixel map function (CsnetMap, CsfMap), so both networks share one counter.
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -125,6 +130,24 @@ CSNET_IO_HD uint8_t img_out_value(const float* z, int W, ImgTap ty, ImgTap tx) {
   return (uint8_t)(s * 255.f);
 }
 
+// CSF+Res2Net's test path (CSF+Res2Net/dataset/dataset.py:83-96 load_image_test, solver.py:62-78 test): no resize on either side.
+// Input channel c of a uint8 value u: numpy's three roundings, `in_ = f32(im) / 255` in fp32, then `in_ -= mean` and `in_ /= std`
+// with float64 mean / std, each computed in float64 and stored back into the fp32 array.
+CSNET_IO_HD float img_csf_in_value(uint8_t u, double mean, double stdv) {
+  const float a = (float)u / 255.f;
+  const float b = (float)((double)a - mean);
+  return (float)((double)b / stdv);
+}
+
+// Map byte of a sigmoid value s: `255 * pred` in fp32, then cv2.imwrite's convertTo(CV_8U), i.e. saturate(round half to even).
+// A NaN gives 0, as cvRound's INT_MIN saturates.
+CSNET_IO_HD uint8_t img_csf_out_byte(float s) {
+  const float r = rintf(255.f * s);
+  return r >= 255.f ? (uint8_t)255 : (r > 0.f ? (uint8_t)r : (uint8_t)0);
+}
+
+CSNET_IO_HD uint8_t img_csf_out_value(float z) { return img_csf_out_byte(img_sigmoid(z)); }
+
 #ifndef CSNET_HOST_EMU
 constexpr int kImgThreads = 256;          // also the x / 255 table's length
 constexpr int kImgRows = 4;               // output rows per block of resize_in_u8_kernel
@@ -164,8 +187,23 @@ __global__ void __launch_bounds__(kImgThreads) resize_in_u8_kernel(const uint8_t
   }
 }
 
+// Map byte at pixel (oy, ox) of an h x w map from one image's logits plane zn [H][W]: the two per-pixel map functions the map and
+// SalMetric kernels are instantiated with.
+struct CsnetMap {            // CSNet/test.py: sigmoid, skimage resize back to (h, w), truncation
+  __device__ __forceinline__ uint8_t operator()(const float* zn, int H, int W, int h, int w, int oy, int ox) const {
+    return img_out_value(zn, W, img_tap(oy, H, h), img_tap(ox, W, w));
+  }
+};
+
+struct CsfMap {              // CSF+Res2Net solver.test: the logits are at the image's size (h, w == H, W), sigmoid, round to even
+  __device__ __forceinline__ uint8_t operator()(const float* zn, int, int W, int, int, int oy, int ox) const {
+    return img_csf_out_value(zn[(int64_t)oy * W + ox]);
+  }
+};
+
 // fp32 logits [N,1,H,W] -> each image's uint8 map [h][w] at its dst_off.  Grid: (blocks per image, image); each block
 // grid-strides over its image's pixels.
+template <class Map>
 __global__ void __launch_bounds__(kImgThreads) resize_out_u8_kernel(const float* __restrict__ z, int H, int W,
                                                                    const csnet_image_geom* __restrict__ geom, uint8_t* __restrict__ y) {
   const int n = blockIdx.y;
@@ -175,14 +213,15 @@ __global__ void __launch_bounds__(kImgThreads) resize_out_u8_kernel(const float*
   const int64_t hw = (int64_t)g.h * g.w;
   for (int64_t p = (int64_t)blockIdx.x * kImgThreads + threadIdx.x; p < hw; p += (int64_t)gridDim.x * kImgThreads) {
     const int oy = (int)p / g.w, ox = (int)p - oy * g.w;     // h * w < 2^31
-    out[p] = img_out_value(zn, W, img_tap(oy, H, g.h), img_tap(ox, W, g.w));
+    out[p] = Map()(zn, H, W, g.h, g.w, oy, ox);
   }
 }
 
-// SalMetric counts (sal_metric.cpp:86-120) of each image's map as resize_out_u8_kernel computes it, against the image's uint8 GT
+// SalMetric counts (sal_metric.cpp:86-120) of each image's map as resize_out_u8_kernel<Map> computes it, against the image's uint8 GT
 // [h][w] at m + dst_off; the map is stored at y + dst_off only when y is non-null.  Grid as resize_out_u8_kernel.  Each warp counts
 // into its own shared histograms (a saliency map piles most pixels into a few bins), the block adds them to image n's global ones
 // with integer atomics: the counts are exact and do not depend on the grid or the batch.  hist_all / hist_pos / abs_sum start at 0.
+template <class Map>
 __global__ void __launch_bounds__(kImgThreads) salmetric_images_u8_kernel(const float* __restrict__ z, int H, int W,
                                                                          const csnet_image_geom* __restrict__ geom,
                                                                          const uint8_t* __restrict__ m, uint8_t* __restrict__ y,
@@ -205,7 +244,7 @@ __global__ void __launch_bounds__(kImgThreads) salmetric_images_u8_kernel(const 
   unsigned long long d = 0;
   for (int64_t p = (int64_t)blockIdx.x * kImgThreads + threadIdx.x; p < hw; p += (int64_t)gridDim.x * kImgThreads) {
     const int oy = (int)p / g.w, ox = (int)p - oy * g.w;     // h * w < 2^31
-    const uint8_t q = img_out_value(zn, W, img_tap(oy, H, g.h), img_tap(ox, W, g.w));
+    const uint8_t q = Map()(zn, H, W, g.h, g.w, oy, ox);
     if (y) y[g.dst_off + p] = q;
     const int t = gt[p];
     atomicAdd(&wa[q], 1u);
@@ -260,6 +299,19 @@ __global__ void __launch_bounds__(kImgThreads) train_batch_u8_kernel(const uint8
   }
 }
 
+// CSF+Res2Net network input: N images of one size H x W, each packed uint8 HWC at its src_off -> fp32 [N,3,H,W]
+// (img_csf_in_value).  Grid: (pixel blocks, image); a thread reads one pixel's 3 bytes and writes it to the 3 planes.
+__global__ void __launch_bounds__(kImgThreads) csf_input_u8_kernel(const uint8_t* __restrict__ x, const csnet_image_geom* __restrict__ geom,
+                                                                  int H, int W, const __grid_constant__ ImgNorm A, float* __restrict__ y) {
+  const int n = blockIdx.y;
+  const int64_t hw = (int64_t)H * W, p = (int64_t)blockIdx.x * kImgThreads + threadIdx.x;
+  if (p >= hw) return;
+  const uint8_t* px = x + geom[n].src_off + 3 * p;
+  float* yn = y + (int64_t)n * 3 * hw + p;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) yn[c * hw] = img_csf_in_value(px[c], A.mean[c], A.std[c]);
+}
+
 constexpr int kMaeThreads = 512;
 
 // Validation MAE per image (train.py:262-279) from fp32 logits [N,1,H,W] and each image's uint8 GT [h][w] at its dst_off.  One block
@@ -297,6 +349,12 @@ inline ImgNorm img_norm(const float* mean, const float* stdv) {
   return A;
 }
 
+inline ImgNorm img_norm(const double* mean, const double* stdv) {
+  ImgNorm A{};
+  for (int c = 0; c < 3; ++c) { A.mean[c] = mean[c]; A.std[c] = stdv[c]; }
+  return A;
+}
+
 inline void launch_resize_in(const uint8_t* x, const csnet_image_geom* geom, int N, int H, int W, const ImgNorm& A, float* y,
                              cudaStream_t stream) {
   resize_in_u8_kernel<<<dim3((unsigned)((H + kImgRows - 1) / kImgRows), (unsigned)N), kImgThreads, 0, stream>>>(x, geom, H, W, A, y);
@@ -304,18 +362,26 @@ inline void launch_resize_in(const uint8_t* x, const csnet_image_geom* geom, int
 
 // The map sizes live on the device, so the grid is sized from the batch alone: about 32 blocks per SM in all, which keeps the
 // SMs busy to the end of a batch whose images differ in size; blocks past a small image's end exit at once.
+template <class Map = CsnetMap>
 inline void launch_resize_out(const float* z, int N, int H, int W, const csnet_image_geom* geom, uint8_t* y, int num_sms,
                               cudaStream_t stream) {
   const int bx = (32 * num_sms + N - 1) / N;
-  resize_out_u8_kernel<<<dim3((unsigned)bx, (unsigned)N), kImgThreads, 0, stream>>>(z, H, W, geom, y);
+  resize_out_u8_kernel<Map><<<dim3((unsigned)bx, (unsigned)N), kImgThreads, 0, stream>>>(z, H, W, geom, y);
 }
 
+template <class Map = CsnetMap>
 inline void launch_salmetric_images(const float* z, int N, int H, int W, const csnet_image_geom* geom, const uint8_t* m, uint8_t* y,
                                     uint32_t* hist_all, uint32_t* hist_pos, unsigned long long* abs_sum, int num_sms, cudaStream_t stream) {
   static_assert(kImgThreads == 256, "one histogram bin per thread");
   const int bx = (32 * num_sms + N - 1) / N;
-  salmetric_images_u8_kernel<<<dim3((unsigned)bx, (unsigned)N), kImgThreads, 0, stream>>>(z, H, W, geom, m, y, hist_all, hist_pos,
-                                                                                          abs_sum);
+  salmetric_images_u8_kernel<Map><<<dim3((unsigned)bx, (unsigned)N), kImgThreads, 0, stream>>>(z, H, W, geom, m, y, hist_all, hist_pos,
+                                                                                               abs_sum);
+}
+
+inline void launch_csf_input(const uint8_t* x, const csnet_image_geom* geom, int N, int H, int W, const ImgNorm& A, float* y,
+                             cudaStream_t stream) {
+  const int64_t bx = ((int64_t)H * W + kImgThreads - 1) / kImgThreads;
+  csf_input_u8_kernel<<<dim3((unsigned)bx, (unsigned)N), kImgThreads, 0, stream>>>(x, geom, H, W, A, y);
 }
 
 inline void launch_train_batch(const uint8_t* x, const uint8_t* m, const csnet_image_geom* geom, const csnet_train_sample* samples, int N,

@@ -1428,6 +1428,46 @@ int csnet_salmetric_images_u8(const float* logits, int32_t N, int32_t H, int32_t
   return CSNET_OK;
 }
 
+int csnet_csf_input_u8(const uint8_t* x_packed, const csnet_image_geom* geom, int32_t N, int32_t H, int32_t W, const double* mean,
+                       const double* stdv, float* x_nchw, void* stream) {
+  if (!x_packed || !geom || !mean || !stdv || !x_nchw) return fail(CSNET_E_INVALID, "csnet_csf_input_u8: null argument");
+  if (N <= 0 || N > 65535 || H <= 0 || W <= 0 || H > csnet::kMaxImageSide || W > csnet::kMaxImageSide)
+    return fail(CSNET_E_INVALID, "csnet_csf_input_u8: N outside [1, 65535] or H, W outside [1, 32767]");
+  csnet::launch_csf_input(x_packed, geom, N, H, W, csnet::img_norm(mean, stdv), x_nchw, (cudaStream_t)stream);
+  CU_CHECK(cudaGetLastError());
+  return CSNET_OK;
+}
+
+int csnet_csf_maps_u8(const float* logits, int32_t N, int32_t H, int32_t W, const csnet_image_geom* geom, uint8_t* y_packed, void* stream) {
+  if (!logits || !geom || !y_packed) return fail(CSNET_E_INVALID, "csnet_csf_maps_u8: null argument");
+  if (N <= 0 || N > 65535 || H <= 0 || W <= 0 || H > csnet::kMaxImageSide || W > csnet::kMaxImageSide)
+    return fail(CSNET_E_INVALID, "csnet_csf_maps_u8: N outside [1, 65535] or H, W outside [1, 32767]");
+  int dev = 0, sms = 0;
+  CU_CHECK(cudaGetDevice(&dev));
+  CU_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  csnet::launch_resize_out<csnet::CsfMap>(logits, N, H, W, geom, y_packed, sms, (cudaStream_t)stream);
+  CU_CHECK(cudaGetLastError());
+  return CSNET_OK;
+}
+
+int csnet_salmetric_csf_u8(const float* logits, int32_t N, int32_t H, int32_t W, const csnet_image_geom* geom, const uint8_t* m_packed,
+                           uint8_t* y_packed, uint32_t* hist_all, uint32_t* hist_pos, unsigned long long* abs_sum, void* stream) {
+  if (!logits || !geom || !m_packed || !hist_all || !hist_pos || !abs_sum)
+    return fail(CSNET_E_INVALID, "csnet_salmetric_csf_u8: null argument");
+  if (N <= 0 || N > 65535 || H <= 0 || W <= 0 || H > csnet::kMaxImageSide || W > csnet::kMaxImageSide)
+    return fail(CSNET_E_INVALID, "csnet_salmetric_csf_u8: N outside [1, 65535] or H, W outside [1, 32767]");
+  cudaStream_t st = (cudaStream_t)stream;
+  int dev = 0, sms = 0;
+  CU_CHECK(cudaGetDevice(&dev));
+  CU_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  CU_CHECK(cudaMemsetAsync(hist_all, 0, (size_t)N * 256 * sizeof(uint32_t), st));
+  CU_CHECK(cudaMemsetAsync(hist_pos, 0, (size_t)N * 256 * sizeof(uint32_t), st));
+  CU_CHECK(cudaMemsetAsync(abs_sum, 0, (size_t)N * sizeof(unsigned long long), st));
+  csnet::launch_salmetric_images<csnet::CsfMap>(logits, N, H, W, geom, m_packed, y_packed, hist_all, hist_pos, abs_sum, sms, st);
+  CU_CHECK(cudaGetLastError());
+  return CSNET_OK;
+}
+
 int csnet_train_batch_u8(const uint8_t* x_packed, const uint8_t* m_packed, const csnet_image_geom* geom, const csnet_train_sample* samples,
                          int32_t N, int32_t H, int32_t W, const float* mean, const float* stdv, float* x_nchw, float* target, void* stream) {
   if (!x_packed || !m_packed || !geom || !samples || !mean || !stdv || !x_nchw || !target)

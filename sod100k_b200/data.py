@@ -180,12 +180,19 @@ class SalImages:
         mask by csnet_salmetric_images_u8.  Only the counts, 2 x 256 + 1 numbers per image, come to the host, where SalMetric.add_images
         turns them into scores, adding the images in input order as sal_metric.cpp does.  Returns SalMetric.compute()'s dict (max_f,
         mean_f, precision, recall, mean_precision, mean_recall, mae, argmax); with maps=True, (scores, maps) where maps are each
-        image's uint8 [h, w] map on the device, in input order."""
-        from .engine import image_runs
+        image's uint8 [h, w] map on the device, in input order.
+
+        A CSFNet `model` is CSF+Res2Net/solver.py:test followed by the same SalMetric: every image at its own size (size must be None;
+        the reference never resizes), grouped by exact size, and scored on CSFNet.forward_images_u8's maps (csnet_salmetric_csf_u8).
+        mean / std go to its input kernel as doubles."""
+        from .engine import exact_size, image_runs, native_size
+        from .networks.csf_res2net import CSFNet
         from .salmetric import SalMetric
 
-        eng = model.engine()
-        order, runs = image_runs(self.sizes, size, batch)
+        csf = isinstance(model, CSFNet)
+        if csf and size is not None:
+            raise ValueError("CSF+Res2Net evaluates every image at its own size: size must be None")
+        order, runs = image_runs(self.sizes, size, batch, key=exact_size if csf else native_size)
         g = self._upload(self.geom_host[order])
         N = len(self)
         hist_all = torch.empty((N, 256), dtype=torch.int32, device=self.device)
@@ -193,12 +200,16 @@ class SalImages:
         abs_sum = torch.empty(N, dtype=torch.int64, device=self.device)
         y = torch.empty(self.m.numel(), dtype=torch.uint8, device=self.device) if maps else None
         stream = self._stream()
+        count = runtime.salmetric_csf_u8 if csf else runtime.salmetric_images_u8
 
         def score(logits, a, b, H, W, g_run):
-            runtime.salmetric_images_u8(logits.data_ptr(), b - a, H, W, g_run, self.m.data_ptr(), y.data_ptr() if maps else 0,
-                                        hist_all[a].data_ptr(), hist_pos[a].data_ptr(), abs_sum[a].data_ptr(), stream)
+            count(logits.data_ptr(), b - a, H, W, g_run, self.m.data_ptr(), y.data_ptr() if maps else 0,
+                  hist_all[a].data_ptr(), hist_pos[a].data_ptr(), abs_sum[a].data_ptr(), stream)
 
-        eng.run_packed_images(self.x, g, runs, size is None, mean, std, score)
+        if csf:
+            model.run_packed_images(self.x, g, runs, mean, std, score)
+        else:
+            model.engine().run_packed_images(self.x, g, runs, size is None, mean, std, score)
         inv = np.argsort(np.asarray(order, np.int64))
         ha, hp, ad = (t.cpu().numpy()[inv] for t in (hist_all, hist_pos, abs_sum))
         hw = self.sizes[:, 0] * self.sizes[:, 1]

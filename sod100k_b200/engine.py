@@ -35,15 +35,21 @@ def native_size(h: int, w: int) -> Tuple[int, int]:
     return h, w
 
 
-def image_runs(sizes: Sequence, size: Optional[Tuple[int, int]], batch: Optional[int]):
+def exact_size(h: int, w: int) -> Tuple[int, int]:
+    """The network input of an h x w image in CSF+Res2Net's solver.test: the image itself, whatever its size."""
+    return h, w
+
+
+def image_runs(sizes: Sequence, size: Optional[Tuple[int, int]], batch: Optional[int], key=native_size):
     """How forward_images_u8 and SalImages.evaluate cut a set of (h, w) images into network runs.  Returns (order, runs): `order` lists
     the images in run order, and each run (a, b, H, W) takes order[a:b] at the network size H x W.  size=(H, W) keeps the input order
-    and runs everything at that size; size=None groups the images by native_size, in ascending padded size so that one pass meets each
-    size once.  No run holds more than `batch` images (None: no limit)."""
+    and runs everything at that size; size=None groups the images by key(h, w) (native_size for CSNet, exact_size for CSF+Res2Net),
+    in ascending network size so that one pass meets each size once, keeping the input order within a size.  No run holds more than
+    `batch` images (None: no limit)."""
     if batch is not None and int(batch) < 1:
         raise ValueError(f"batch must be at least 1, got {batch}")
     hw = [(int(h), int(w)) for h, w in sizes]
-    net = [native_size(h, w) for h, w in hw] if size is None else [(int(size[0]), int(size[1]))] * len(hw)
+    net = [key(h, w) for h, w in hw] if size is None else [(int(size[0]), int(size[1]))] * len(hw)
     order = sorted(range(len(hw)), key=lambda i: net[i]) if size is None else list(range(len(hw)))
     step = len(hw) if batch is None else int(batch)
     runs: List[Tuple[int, int, int, int]] = []

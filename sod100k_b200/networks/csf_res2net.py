@@ -16,6 +16,7 @@ from __future__ import annotations
 import math
 from collections import OrderedDict
 
+import numpy as np
 import torch
 import torch.nn as nn
 from torch.nn import init
@@ -174,6 +175,7 @@ class CSFNet(nn.Module):
         self._plans = OrderedDict()              # (h, w, precision, device) -> head plan, least recently used first
         self._plan_version = {}
         self.plan_budget = PLAN_BUDGET
+        self._pinned_images = None               # forward_images_u8's packed host input, reused across calls
 
     def set_precision(self, dtype: str):
         self.precision = dtype
@@ -181,7 +183,7 @@ class CSFNet(nn.Module):
 
     def __getstate__(self):                      # device plans (ctypes handles) never travel with a copy / pickle
         d = dict(self.__dict__)
-        d["_plans"], d["_plan_version"] = OrderedDict(), {}
+        d["_plans"], d["_plan_version"], d["_pinned_images"] = OrderedDict(), {}, None
         return d
 
     def __deepcopy__(self, memo):
@@ -190,9 +192,9 @@ class CSFNet(nn.Module):
         new = self.__class__.__new__(self.__class__)
         memo[id(self)] = new
         for k, v in self.__dict__.items():
-            if k not in ("_plans", "_plan_version"):
+            if k not in ("_plans", "_plan_version", "_pinned_images"):
                 new.__dict__[k] = copy.deepcopy(v, memo)
-        new._plans, new._plan_version = OrderedDict(), {}
+        new._plans, new._plan_version, new._pinned_images = OrderedDict(), {}, None
         return new
 
     def head_state(self):
@@ -214,20 +216,33 @@ class CSFNet(nn.Module):
             from .. import modular_r
 
             return modular_r.csf_head(self, self.base(x.float()), x.shape[2:])
+        self._check_inference()
+        feats = self.backbone(x.float())
+        return self._run_head(feats, x.shape, x.device, self._head_version())
+
+    def _check_inference(self):
         if self.training:
             raise NotImplementedError("CSF+Res2Net runs inference under model.eval() and torch.no_grad(), and trains with autograd "
                                       "recording (grad enabled, parameters or input requiring grad)")
-        n, _, h, w = x.shape
+
+    def _head_version(self) -> int:
+        """Version stamp of the head's parameters and buffers.  It reads a checksum back to the host, so a pass over many runs takes
+        it once."""
+        from ..engine import param_version
+
+        return param_version([t for k, t in list(self.named_parameters()) + list(self.named_buffers()) if not k.startswith("base.")])
+
+    def _run_head(self, feats, shape, device, ver: int) -> torch.Tensor:
+        """The head on backbone features of a batch of input `shape` (n, 3, h, w): fp32 logits [n, 1, h, w] on the current stream."""
+        n, _, h, w = shape
         # any (h, w): the head program resizes between the backbone's ceil(h / 2) stages as the reference does.  One plan per size
         # lives in an LRU cache whose arenas `plan_budget` bounds (the plan in use stays even when it alone exceeds the budget)
-        feats = self.backbone(x.float())
-        key = (h, w, self.precision, x.device.index or 0)
+        key = (h, w, self.precision, device.index or 0)
         plan = self._plans.get(key)
         # the head plan folds the head's parameters at creation: re-fold when they change (load_state_dict, weights_init,
         # `.data` writes — same version stamp as the CSNet engine), so head and backbone never run on different weights
-        from ..engine import param_version, trim_plans
+        from ..engine import trim_plans
 
-        ver = param_version([t for k, t in list(self.named_parameters()) + list(self.named_buffers()) if not k.startswith("base.")])
         if plan is None or plan.max_batch < n:
             prog = compiler_r.compile_csf_head(self.head_state(), [tuple(f.shape[1:]) for f in feats], h, w, self.precision)
             if plan is not None:
@@ -236,7 +251,7 @@ class CSFNet(nn.Module):
         elif self._plan_version.get(key) != ver:
             prog = compiler_r.compile_csf_head(self.head_state(), [tuple(f.shape[1:]) for f in feats], h, w, self.precision)
             if prog.signature() == plan.prog.signature():
-                plan.set_blob(prog.blob, torch.cuda.current_stream(x.device).cuda_stream)
+                plan.set_blob(prog.blob, torch.cuda.current_stream(device).cuda_stream)
                 plan.prog = prog
             else:
                 mb = plan.max_batch
@@ -245,9 +260,87 @@ class CSFNet(nn.Module):
         self._plan_version[key] = ver
         self._plans.move_to_end(key)
         trim_plans(self._plans, self.plan_budget, self._plan_version, keep=key)
-        y = torch.empty((n, 1, h, w), dtype=torch.float32, device=x.device)
-        plan.run(n, [f.data_ptr() for f in feats] + [y.data_ptr()], torch.cuda.current_stream(x.device).cuda_stream)
+        y = torch.empty((n, 1, h, w), dtype=torch.float32, device=device)
+        plan.run(n, [f.data_ptr() for f in feats] + [y.data_ptr()], torch.cuda.current_stream(device).cuda_stream)
         return y
+
+    IMAGENET_MEAN, IMAGENET_STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)          # CSF+Res2Net/dataset/dataset.py:load_image_test
+
+    def run_packed_images(self, x_packed: torch.Tensor, geom_dev: torch.Tensor, runs, mean, std, consume) -> None:
+        """The device side of forward_images_u8 and SalImages.evaluate: for each run (a, b, H, W) of image_runs(..., key=exact_size),
+        the H x W images of entries a..b-1 of the device geometry table `geom_dev` become the network input (csnet_csf_input_u8), go
+        through the backbone and the head as forward runs them, and consume(logits, a, b, H, W, geometry address of entry a) takes the
+        fp32 logits [b - a, 1, H, W], on the current stream.  Runs under torch.no_grad(); a net in training mode raises."""
+        self._check_inference()
+        dev = x_packed.device
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        with torch.no_grad():
+            ver = self._head_version()
+            for a, b, H, W in runs:
+                n = b - a
+                g = geom_dev.data_ptr() + a * runtime.GEOM_DTYPE.itemsize
+                x = torch.empty((n, 3, H, W), dtype=torch.float32, device=dev)
+                runtime.csf_input_u8(x_packed.data_ptr(), g, n, H, W, mean, std, x.data_ptr(), stream)
+                consume(self._run_head(self.backbone(x), x.shape, dev, ver), a, b, H, W, g)
+
+    @staticmethod
+    def _image_u8(im, i: int) -> torch.Tensor:
+        """One uint8 RGB [h, w, 3] image as a tensor; a gray [h, w] one is replicated to 3 channels (cv2.IMREAD_COLOR does)."""
+        if isinstance(im, np.ndarray):
+            im = torch.from_numpy(np.ascontiguousarray(im))
+        if not isinstance(im, torch.Tensor) or im.dtype != torch.uint8 or not (im.dim() == 2 or (im.dim() == 3 and im.shape[2] == 3)):
+            raise ValueError(f"image {i}: expected a uint8 [h, w, 3] or [h, w] array or tensor, got "
+                             f"{getattr(im, 'dtype', type(im).__name__)} {tuple(getattr(im, 'shape', ()))}")
+        if not (1 <= im.shape[0] <= 32767 and 1 <= im.shape[1] <= 32767):
+            raise ValueError(f"image {i}: h and w must lie in [1, 32767], got {tuple(im.shape[:2])}")
+        return im.unsqueeze(2).expand(-1, -1, 3) if im.dim() == 2 else im
+
+    def forward_images_u8(self, images, batch: int = None, device: int = 0, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+        """CSF+Res2Net/solver.py:test for a list of images of any sizes: each RGB uint8 image goes in at its own size, normalised as
+        dataset.load_image_test does, and its map is the uint8 [h, w] that solver.test writes with cv2.imwrite (255 * sigmoid, rounded
+        half to even).  Returns the maps in input order.  Images are grouped by exact size (padding would change the maps); no run
+        takes more than `batch` images (None: all images of one size in one run).
+
+        `images` are uint8 [h, w, 3] or gray [h, w] numpy arrays or CPU tensors (packed into one pinned buffer reused across calls and
+        copied to device `device` once; the maps are views of one pinned buffer), or all CUDA tensors on one device (the maps stay on
+        that device)."""
+        from ..engine import exact_size, image_runs
+
+        imgs = [self._image_u8(im, i) for i, im in enumerate(images)]
+        if not imgs:
+            return []
+        if len({t.device for t in imgs}) > 1:
+            raise ValueError("forward_images_u8 takes host images or CUDA images of one device, not a mix")
+        order, runs = image_runs([t.shape[:2] for t in imgs], None, batch, key=exact_size)
+        imgs = [imgs[i] for i in order]
+        geom = runtime.image_geometry([t.shape[:2] for t in imgs])
+        hw = (geom["h"].astype(np.int64) * geom["w"]).tolist()
+        total = sum(hw)
+        host = not imgs[0].is_cuda
+        dev = torch.device("cuda", device) if host else imgs[0].device
+        if host:
+            if self._pinned_images is None or self._pinned_images.numel() < 3 * total:
+                self._pinned_images = torch.empty(3 * total, dtype=torch.uint8, pin_memory=True)
+            x = self._pinned_images[:3 * total]
+            torch.cat([t.reshape(-1) for t in imgs], out=x)
+            x = x.to(dev, non_blocking=True)
+        else:
+            x = torch.cat([t.reshape(-1) for t in imgs])
+        g = torch.from_numpy(geom.view(np.uint8)).pin_memory().to(dev, non_blocking=True)
+        y = torch.empty(total, dtype=torch.uint8, device=dev)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+
+        def store(logits, a, b, H, W, g_run):
+            runtime.csf_maps_u8(logits.data_ptr(), b - a, H, W, g_run, y.data_ptr(), stream)
+
+        self.run_packed_images(x, g, runs, mean, std, store)
+        if host:
+            y = torch.empty(total, dtype=torch.uint8, pin_memory=True).copy_(y, non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()
+        maps = [None] * len(imgs)
+        for i, o, n, t in zip(order, geom["dst_off"].tolist(), hw, imgs):
+            maps[i] = y[o:o + n].view(t.shape[0], t.shape[1])
+        return maps
 
 
 def build_model():

@@ -13,7 +13,7 @@ from . import ir
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libcsnet_b200.so")
-ABI_VERSION = 10
+ABI_VERSION = 11
 PARAM_EPOCH = 0      # bumped by in-place parameter updates that bypass torch's version counters (FusedAdam)
 _lib = None
 
@@ -26,7 +26,8 @@ SYMBOLS = ("csnet_abi_version", "csnet_last_error", "csnet_device_count", "csnet
            "csnet_train_dw_conv", "csnet_train_dw_wgrad", "csnet_train_dw_bwd", "csnet_train_mix_fwd", "csnet_train_mix_dgrad",
            "csnet_train_mix_wgrad", "csnet_train_pool_fwd", "csnet_train_pool_bwd", "csnet_slim_gather", "csnet_train_bce", "csnet_train_adam", "csnet_salmetric_hist",
            "csnet_train_conv_plan", "csnet_train_conv_fwd", "csnet_train_conv_dgrad", "csnet_train_conv_wgrad", "csnet_train_bias_grad",
-           "csnet_train_gn_stats", "csnet_train_gn_prelu_fwd", "csnet_train_gn_prelu_bwd", "csnet_train_resize_fwd", "csnet_train_resize_bwd")
+           "csnet_train_gn_stats", "csnet_train_gn_prelu_fwd", "csnet_train_gn_prelu_bwd", "csnet_train_resize_fwd", "csnet_train_resize_bwd",
+           "csnet_csf_input_u8", "csnet_csf_maps_u8", "csnet_salmetric_csf_u8")
 
 
 class EngineError(RuntimeError):
@@ -118,6 +119,13 @@ def load_library(path: Optional[str] = None):
                                          C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_void_p, C.c_void_p, C.c_void_p]
     lib.csnet_val_mae_u8.restype = C.c_int
     lib.csnet_val_mae_u8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.csnet_csf_input_u8.restype = C.c_int
+    lib.csnet_csf_input_u8.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double),
+                                       C.POINTER(C.c_double), C.c_void_p, C.c_void_p]
+    lib.csnet_csf_maps_u8.restype = C.c_int
+    lib.csnet_csf_maps_u8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.csnet_salmetric_csf_u8.restype = C.c_int
+    lib.csnet_salmetric_csf_u8.argtypes = lib.csnet_salmetric_images_u8.argtypes
     lib.csnet_slim_gather.restype = C.c_int
     lib.csnet_slim_gather.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     lib.csnet_train_last_error.restype = C.c_char_p
@@ -155,6 +163,29 @@ def salmetric_images_u8(logits_ptr: int, N: int, H: int, W: int, geom_dev_ptr: i
     lib = load_library()
     _check(lib, lib.csnet_salmetric_images_u8(logits_ptr, int(N), int(H), int(W), geom_dev_ptr, m_packed_ptr, y_packed_ptr or None,
                                               hist_all_ptr, hist_pos_ptr, abs_sum_ptr, stream), "csnet_salmetric_images_u8")
+
+
+def csf_input_u8(x_packed_ptr: int, geom_dev_ptr: int, N: int, H: int, W: int, mean, std, x_nchw_ptr: int, stream: int = 0):
+    """Device to device: N packed uint8 images of size H x W -> fp32 [N,3,H,W] as CSF+Res2Net's load_image_test computes it, mean /
+    std taken as doubles (csnet_csf_input_u8)."""
+    lib = load_library()
+    m, s_ = (C.c_double * 3)(*mean), (C.c_double * 3)(*std)
+    _check(lib, lib.csnet_csf_input_u8(x_packed_ptr, geom_dev_ptr, int(N), int(H), int(W), m, s_, x_nchw_ptr, stream), "csnet_csf_input_u8")
+
+
+def csf_maps_u8(logits_ptr: int, N: int, H: int, W: int, geom_dev_ptr: int, y_packed_ptr: int, stream: int = 0):
+    """Device to device: fp32 logits [N,1,H,W] at the images' own size -> each image's uint8 map at its dst_off, rounded as
+    CSF+Res2Net's solver.test writes it (csnet_csf_maps_u8)."""
+    lib = load_library()
+    _check(lib, lib.csnet_csf_maps_u8(logits_ptr, int(N), int(H), int(W), geom_dev_ptr, y_packed_ptr, stream), "csnet_csf_maps_u8")
+
+
+def salmetric_csf_u8(logits_ptr: int, N: int, H: int, W: int, geom_dev_ptr: int, m_packed_ptr: int, y_packed_ptr: int,
+                     hist_all_ptr: int, hist_pos_ptr: int, abs_sum_ptr: int, stream: int = 0):
+    """salmetric_images_u8 for the maps csf_maps_u8 writes (csnet_salmetric_csf_u8)."""
+    lib = load_library()
+    _check(lib, lib.csnet_salmetric_csf_u8(logits_ptr, int(N), int(H), int(W), geom_dev_ptr, m_packed_ptr, y_packed_ptr or None,
+                                           hist_all_ptr, hist_pos_ptr, abs_sum_ptr, stream), "csnet_salmetric_csf_u8")
 
 
 def train_batch_u8(x_packed_ptr: int, m_packed_ptr: int, geom_dev_ptr: int, samples_dev_ptr: int, N: int, H: int, W: int, mean, std,
