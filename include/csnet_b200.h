@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define CSNET_ABI_VERSION 11
+#define CSNET_ABI_VERSION 12
 
 enum { CSNET_F32 = 0, CSNET_F16 = 1, CSNET_BF16 = 2 };
 
@@ -295,6 +295,14 @@ int csnet_val_mae_u8(const float* logits, int32_t N, int32_t H, int32_t W, const
 int csnet_csf_input_u8(const uint8_t* x_packed, const csnet_image_geom* geom, int32_t N, int32_t H, int32_t W, const double* mean,
                        const double* std, float* x_nchw, void* stream);
 
+/* Training samples (CSF+Res2Net/solver.py:81-127 with dataset.py:23-33, 69-114): sample n is image samples[n].image of the packed set,
+ * flipped along W when samples[n].flip is 1 (cv_random_flip), never cropped or resized.  x_nchw fp32 [N,3,H,W] as csnet_csf_input_u8
+ * computes it; target fp32 [N,1,H,W] = f32(m) / 255.f from the mask at m_packed + dst_off (load_sal_label).  samples DEVICE [N] with
+ * y0 = x0 = 0, h = H, w = W, flip 0 or 1; mean / std host double[3]. */
+int csnet_csf_train_batch_u8(const uint8_t* x_packed, const uint8_t* m_packed, const csnet_image_geom* geom, const csnet_train_sample* samples,
+                             int32_t N, int32_t H, int32_t W, const double* mean, const double* std, float* x_nchw, float* target,
+                             void* stream);
+
 /* Logits fp32 [N,1,H,W] -> each image's map at y_packed + dst_off, q = saturate(rint(255.f * sigmoid(z))) with round half to even
  * (cv2.imwrite of solver.test's fp32 array) and sigmoid = 1.f / (1.f + expf(-z)) as torch's CUDA kernel computes it. */
 int csnet_csf_maps_u8(const float* logits, int32_t N, int32_t H, int32_t W, const csnet_image_geom* geom, uint8_t* y_packed, void* stream);
@@ -370,6 +378,10 @@ int csnet_slim_gather(const float* src, int32_t Co, int32_t Ci, int32_t kk, cons
                       float* dst, int32_t dCo, int32_t dCi, void* stream);
 /* F.binary_cross_entropy_with_logits (mean) and its gradient * grad_scale (train.py:209). */
 int csnet_train_bce(const float* logits, const float* target, float* dlogits, float* loss, int64_t n, float grad_scale, void* stream);
+/* F.binary_cross_entropy_with_logits(reduction='sum') / divisor (CSF+Res2Net/solver.py:101-102): loss[0] = fp32 sum of the n terms
+ * divided by (float)divisor, dlogits (may be NULL) = (sigmoid(z) - t) * f32(1 / divisor).  Deterministic: per-block partials merged
+ * in a fixed order, no floating-point atomics, the block count a function of n alone.  n >= 1, divisor >= 1. */
+int csnet_train_bce_sum(const float* logits, const float* target, float* dlogits, float* loss, int64_t n, int32_t divisor, void* stream);
 /* torch.optim.Adam step (train.py:108-123) over many tensors: `chunk_table_device` = n_chunks records
  * {float* p; const float* g; float* m; float* v; int32 n; float weight_decay} (40 bytes each). */
 int csnet_train_adam(const void* chunk_table_device, int32_t n_chunks, float lr, float beta1, float beta2, float eps, int32_t step,

@@ -21,6 +21,7 @@
 // CSF+Res2Net's test (CSF+Res2Net/solver.py:62-78, dataset.py:83-96) runs each image at its own size, so neither side resizes:
 //   csf in:  img_csf_in_value, numpy's three fp32 roundings of load_image_test
 //   csf out: img_csf_out_value, cv2.imwrite of the fp32 array 255 * sigmoid: rounded half to even and saturated, not truncated
+//   csf train: `csf in` and img_csf_label_value (m / 255 in fp32), both flipped along W (img_csf_src_col); solver.py:81-127
 // The map and SalMetric kernels are templates on the per-pixel map function (CsnetMap, CsfMap), so both networks share one counter.
 #pragma once
 #include <math.h>
@@ -147,6 +148,14 @@ CSNET_IO_HD uint8_t img_csf_out_byte(float s) {
 }
 
 CSNET_IO_HD uint8_t img_csf_out_value(float z) { return img_csf_out_byte(img_sigmoid(z)); }
+
+// CSF+Res2Net's training sample (dataset.py:23-33 ImageDataTrain.__getitem__, load_image, load_sal_label, cv_random_flip): the image
+// as img_csf_in_value (load_image rounds as load_image_test does), the label `np.array(Image.open(gt), float32) / 255.`, which numpy
+// divides in fp32, and both flipped along W when randint(0, 1) gave 1.  No crop, no resize.
+CSNET_IO_HD float img_csf_label_value(uint8_t u) { return (float)u / 255.f; }
+
+// Stored column of output column x of a w-wide row, flipped (img[:, :, ::-1]) when flip is 1.
+CSNET_IO_HD int img_csf_src_col(int x, int w, int flip) { return flip == 1 ? w - 1 - x : x; }
 
 #ifndef CSNET_HOST_EMU
 constexpr int kImgThreads = 256;          // also the x / 255 table's length
@@ -312,6 +321,28 @@ __global__ void __launch_bounds__(kImgThreads) csf_input_u8_kernel(const uint8_t
   for (int c = 0; c < 3; ++c) yn[c * hw] = img_csf_in_value(px[c], A.mean[c], A.std[c]);
 }
 
+// CSF+Res2Net training batch: sample n is image samples[n].image of the packed set (H x W, as every sample of the call), flipped along
+// W when its flip is 1 -> x fp32 [N,3,H,W] (img_csf_in_value) and target fp32 [N,1,H,W] (img_csf_label_value).  Grid as
+// csf_input_u8_kernel: a thread reads one pixel's 3 image bytes and its mask byte.
+__global__ void __launch_bounds__(kImgThreads) csf_train_batch_u8_kernel(const uint8_t* __restrict__ x, const uint8_t* __restrict__ m,
+                                                                        const csnet_image_geom* __restrict__ geom,
+                                                                        const csnet_train_sample* __restrict__ samples, int H, int W,
+                                                                        const __grid_constant__ ImgNorm A, float* __restrict__ y,
+                                                                        float* __restrict__ target) {
+  const int n = blockIdx.y;
+  const int64_t hw = (int64_t)H * W, p = (int64_t)blockIdx.x * kImgThreads + threadIdx.x;
+  if (p >= hw) return;
+  const csnet_train_sample s = samples[n];
+  const csnet_image_geom g = geom[s.image];
+  const int oy = (int)(p / W), ox = (int)(p - (int64_t)oy * W);
+  const int64_t q = (int64_t)oy * W + img_csf_src_col(ox, W, s.flip);
+  const uint8_t* px = x + g.src_off + 3 * q;
+  float* yn = y + (int64_t)n * 3 * hw + p;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) yn[c * hw] = img_csf_in_value(px[c], A.mean[c], A.std[c]);
+  target[(int64_t)n * hw + p] = img_csf_label_value(m[g.dst_off + q]);
+}
+
 constexpr int kMaeThreads = 512;
 
 // Validation MAE per image (train.py:262-279) from fp32 logits [N,1,H,W] and each image's uint8 GT [h][w] at its dst_off.  One block
@@ -382,6 +413,12 @@ inline void launch_csf_input(const uint8_t* x, const csnet_image_geom* geom, int
                              cudaStream_t stream) {
   const int64_t bx = ((int64_t)H * W + kImgThreads - 1) / kImgThreads;
   csf_input_u8_kernel<<<dim3((unsigned)bx, (unsigned)N), kImgThreads, 0, stream>>>(x, geom, H, W, A, y);
+}
+
+inline void launch_csf_train_batch(const uint8_t* x, const uint8_t* m, const csnet_image_geom* geom, const csnet_train_sample* samples,
+                                   int N, int H, int W, const ImgNorm& A, float* y, float* target, cudaStream_t stream) {
+  const int64_t bx = ((int64_t)H * W + kImgThreads - 1) / kImgThreads;
+  csf_train_batch_u8_kernel<<<dim3((unsigned)bx, (unsigned)N), kImgThreads, 0, stream>>>(x, m, geom, samples, H, W, A, y, target);
 }
 
 inline void launch_train_batch(const uint8_t* x, const uint8_t* m, const csnet_image_geom* geom, const csnet_train_sample* samples, int N,

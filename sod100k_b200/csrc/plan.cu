@@ -1438,6 +1438,19 @@ int csnet_csf_input_u8(const uint8_t* x_packed, const csnet_image_geom* geom, in
   return CSNET_OK;
 }
 
+int csnet_csf_train_batch_u8(const uint8_t* x_packed, const uint8_t* m_packed, const csnet_image_geom* geom, const csnet_train_sample* samples,
+                             int32_t N, int32_t H, int32_t W, const double* mean, const double* stdv, float* x_nchw, float* target,
+                             void* stream) {
+  if (!x_packed || !m_packed || !geom || !samples || !mean || !stdv || !x_nchw || !target)
+    return fail(CSNET_E_INVALID, "csnet_csf_train_batch_u8: null argument");
+  if (N <= 0 || N > 65535 || H <= 0 || W <= 0 || H > csnet::kMaxImageSide || W > csnet::kMaxImageSide)
+    return fail(CSNET_E_INVALID, "csnet_csf_train_batch_u8: N outside [1, 65535] or H, W outside [1, 32767]");
+  csnet::launch_csf_train_batch(x_packed, m_packed, geom, samples, N, H, W, csnet::img_norm(mean, stdv), x_nchw, target,
+                                (cudaStream_t)stream);
+  CU_CHECK(cudaGetLastError());
+  return CSNET_OK;
+}
+
 int csnet_csf_maps_u8(const float* logits, int32_t N, int32_t H, int32_t W, const csnet_image_geom* geom, uint8_t* y_packed, void* stream) {
   if (!logits || !geom || !y_packed) return fail(CSNET_E_INVALID, "csnet_csf_maps_u8: null argument");
   if (N <= 0 || N > 65535 || H <= 0 || W <= 0 || H > csnet::kMaxImageSide || W > csnet::kMaxImageSide)

@@ -12,6 +12,7 @@
 #include <string>
 
 #include "../../include/csnet_b200.h"
+#include "bce_sum.cuh"
 #include "generic_ops.cuh"
 #include "train_fast.cuh"
 
@@ -839,6 +840,15 @@ int csnet_train_bce(const float* logits, const float* target, float* dlogits, fl
   TR_CHECK(cudaMemsetAsync(loss, 0, sizeof(float), (cudaStream_t)stream));
   const int blocks = (int)((n + kT * 8 - 1) / (kT * 8) < 1184 ? (n + kT * 8 - 1) / (kT * 8) : 1184);
   bce_kernel<<<blocks < 1 ? 1 : blocks, kT, 0, (cudaStream_t)stream>>>(logits, target, dlogits, loss, n, 1.f / (float)n, grad_scale);
+  TR_CHECK(cudaGetLastError());
+  return CSNET_OK;
+}
+
+int csnet_train_bce_sum(const float* logits, const float* target, float* dlogits, float* loss, int64_t n, int32_t divisor, void* stream) {
+  if (!logits || !target || !loss || n < 1 || divisor < 1) { t_err = "csnet_train_bce_sum: bad arguments"; return CSNET_E_INVALID; }
+  float* part = nullptr;
+  if (int rc = partial_workspace((size_t)csnet::bce::blocks(n), (cudaStream_t)stream, &part)) return rc;
+  csnet::bce::launch(logits, target, dlogits, part, loss, n, divisor, (cudaStream_t)stream);
   TR_CHECK(cudaGetLastError());
   return CSNET_OK;
 }

@@ -12,6 +12,10 @@ draws them, cross PCIe.  The training loop of train.py becomes
             loss = trainer.step(*ds.train_batch(idx, rng))
 
 and a test set is scored like CSNet/test.py followed by eval.py with `SalImages(images, gts).evaluate(model)`.
+
+CSF+Res2Net trains on the same packed set: `csf_train_batch` builds ImageDataTrain's samples (no crop, no resize, a flip per item)
+and trainer.CSFTrainer runs solver.train's step, gradient accumulation and Adam schedule on them.  The reference skips an image whose
+label differs in size ('IMAGE ERROR'); a SalImages set refuses such a pair when it is packed.
 """
 from __future__ import annotations
 
@@ -43,6 +47,13 @@ def augment_params(rng: random.Random, h: int, w: int) -> Tuple[int, int, int, i
     if rng.random() < P_FLIP:
         flip = 1 if rng.random() < 0.5 else 2
     return row1, col1, h + row2 - row1, w + col2 - col1, flip
+
+
+def csf_flip(rng: random.Random) -> int:
+    """One draw of CSF+Res2Net's cv_random_flip (dataset.py:109-114): random.randint(0, 1), 1 flipping image and label along W.  With
+    num_thread = 1 the reference's DataLoader seeds its worker's `random` module with random.seed(base_seed) at every epoch, base_seed
+    drawn from torch's generator; a random.Random(base_seed) per epoch drawing once per item, in loader order, replays its flips."""
+    return rng.randint(0, 1)
 
 
 def _u8(a, what: str) -> torch.Tensor:
@@ -145,6 +156,38 @@ class SalImages:
         sd = self._upload(s)
         runtime.train_batch_u8(self.x.data_ptr(), self.m.data_ptr(), self.geom.data_ptr(), sd.data_ptr(), N, H, W, mean, std,
                                x.data_ptr(), t.data_ptr(), self._stream())
+        return x, t
+
+    def csf_train_batch(self, indices, rng: Optional[random.Random] = None, flips=None, mean=IMAGENET_MEAN,
+                        std=IMAGENET_STD) -> Tuple[torch.Tensor, torch.Tensor]:
+        """CSF+Res2Net's ImageDataTrain.__getitem__ (dataset.py:23-33) for each index: (x fp32 [N,3,H,W], t fp32 [N,1,H,W]) on the current
+        stream, without a host sync (csnet_csf_train_batch_u8).  The images are never cropped or resized, so every index must name an
+        image of one exact size H x W.  x is load_image's normalisation (img_csf_in_value, mean / std as doubles), t the mask / 255 in
+        fp32 (load_sal_label; a 3-channel GT's channel 0 is the mask the caller packs).  `rng` draws one flip per index with csf_flip,
+        in index order; `flips` gives them instead (0 or 1 each, 1 = 'lr'); neither means no flip.  Mixed sizes, bad flips and bad
+        indices raise ValueError before any device work."""
+        idx = _indices(indices, len(self))
+        if rng is not None and flips is not None:
+            raise ValueError("pass rng or flips, not both")
+        sizes = {(int(self.sizes[i, 0]), int(self.sizes[i, 1])) for i in idx}
+        if len(sizes) != 1:
+            raise ValueError(f"csf_train_batch takes images of one size, got {sorted(sizes)}")
+        if flips is not None:
+            fl = np.asarray(flips)
+            if fl.shape != (len(idx),) or not np.issubdtype(fl.dtype, np.integer) or not np.isin(fl, (0, 1)).all():
+                raise ValueError(f"flips: expected {len(idx)} integers, each 0 or 1, got {fl.dtype} {fl.shape}")
+        elif rng is not None:
+            fl = np.array([csf_flip(rng) for _ in idx], np.int64)
+        else:
+            fl = 0
+        N, (H, W) = len(idx), sizes.pop()
+        s = np.zeros(N, runtime.SAMPLE_DTYPE)
+        s["image"], s["h"], s["w"], s["flip"] = idx, H, W, fl
+        x = torch.empty((N, 3, H, W), dtype=torch.float32, device=self.device)
+        t = torch.empty((N, 1, H, W), dtype=torch.float32, device=self.device)
+        sd = self._upload(s)
+        runtime.csf_train_batch_u8(self.x.data_ptr(), self.m.data_ptr(), self.geom.data_ptr(), sd.data_ptr(), N, H, W, mean, std,
+                                   x.data_ptr(), t.data_ptr(), self._stream())
         return x, t
 
     def val_batch(self, indices, size=(224, 224), mean=IMAGENET_MEAN, std=IMAGENET_STD) -> torch.Tensor:

@@ -13,7 +13,7 @@ from . import ir
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libcsnet_b200.so")
-ABI_VERSION = 11
+ABI_VERSION = 12
 PARAM_EPOCH = 0      # bumped by in-place parameter updates that bypass torch's version counters (FusedAdam)
 _lib = None
 
@@ -27,7 +27,7 @@ SYMBOLS = ("csnet_abi_version", "csnet_last_error", "csnet_device_count", "csnet
            "csnet_train_mix_wgrad", "csnet_train_pool_fwd", "csnet_train_pool_bwd", "csnet_slim_gather", "csnet_train_bce", "csnet_train_adam", "csnet_salmetric_hist",
            "csnet_train_conv_plan", "csnet_train_conv_fwd", "csnet_train_conv_dgrad", "csnet_train_conv_wgrad", "csnet_train_bias_grad",
            "csnet_train_gn_stats", "csnet_train_gn_prelu_fwd", "csnet_train_gn_prelu_bwd", "csnet_train_resize_fwd", "csnet_train_resize_bwd",
-           "csnet_csf_input_u8", "csnet_csf_maps_u8", "csnet_salmetric_csf_u8")
+           "csnet_csf_input_u8", "csnet_csf_maps_u8", "csnet_salmetric_csf_u8", "csnet_csf_train_batch_u8", "csnet_train_bce_sum")
 
 
 class EngineError(RuntimeError):
@@ -122,6 +122,11 @@ def load_library(path: Optional[str] = None):
     lib.csnet_csf_input_u8.restype = C.c_int
     lib.csnet_csf_input_u8.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double),
                                        C.POINTER(C.c_double), C.c_void_p, C.c_void_p]
+    lib.csnet_csf_train_batch_u8.restype = C.c_int
+    lib.csnet_csf_train_batch_u8.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                             C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.csnet_train_bce_sum.restype = C.c_int
+    lib.csnet_train_bce_sum.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p]
     lib.csnet_csf_maps_u8.restype = C.c_int
     lib.csnet_csf_maps_u8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.csnet_salmetric_csf_u8.restype = C.c_int
@@ -171,6 +176,26 @@ def csf_input_u8(x_packed_ptr: int, geom_dev_ptr: int, N: int, H: int, W: int, m
     lib = load_library()
     m, s_ = (C.c_double * 3)(*mean), (C.c_double * 3)(*std)
     _check(lib, lib.csnet_csf_input_u8(x_packed_ptr, geom_dev_ptr, int(N), int(H), int(W), m, s_, x_nchw_ptr, stream), "csnet_csf_input_u8")
+
+
+def csf_train_batch_u8(x_packed_ptr: int, m_packed_ptr: int, geom_dev_ptr: int, samples_dev_ptr: int, N: int, H: int, W: int, mean,
+                       std, x_nchw_ptr: int, target_ptr: int, stream: int = 0):
+    """Device to device: N packed uint8 images and masks of size H x W, each flipped along W when its sample's flip is 1 -> fp32 input
+    [N,3,H,W] and target [N,1,H,W] as CSF+Res2Net's ImageDataTrain computes them, mean / std taken as doubles
+    (csnet_csf_train_batch_u8)."""
+    lib = load_library()
+    m, s_ = (C.c_double * 3)(*mean), (C.c_double * 3)(*std)
+    _check(lib, lib.csnet_csf_train_batch_u8(x_packed_ptr, m_packed_ptr, geom_dev_ptr, samples_dev_ptr, int(N), int(H), int(W), m, s_,
+                                             x_nchw_ptr, target_ptr, stream), "csnet_csf_train_batch_u8")
+
+
+def train_bce_sum(logits_ptr: int, target_ptr: int, dlogits_ptr: int, loss_ptr: int, n: int, divisor: int, stream: int = 0):
+    """Device to device: loss = BCE-with-logits summed over n elements / divisor, dlogits = (sigmoid(z) - t) * f32(1 / divisor)
+    (csnet_train_bce_sum; dlogits_ptr may be 0)."""
+    lib = load_library()
+    rc = lib.csnet_train_bce_sum(logits_ptr, target_ptr, dlogits_ptr or None, loss_ptr, int(n), int(divisor), stream)
+    if rc != 0:
+        raise EngineError(f"csnet_train_bce_sum failed ({rc}): {lib.csnet_train_last_error().decode()}")
 
 
 def csf_maps_u8(logits_ptr: int, N: int, H: int, W: int, geom_dev_ptr: int, y_packed_ptr: int, stream: int = 0):

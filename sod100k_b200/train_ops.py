@@ -301,6 +301,28 @@ class BceFn(torch.autograd.Function):
         return dl * g, None
 
 
+class BceSumFn(torch.autograd.Function):
+    """F.binary_cross_entropy_with_logits(logits, target, reduction='sum') / divisor (CSF+Res2Net/solver.py:101-102), the sum
+    reduced in a fixed order (csnet_train_bce_sum): the same bits on every run."""
+
+    @staticmethod
+    def forward(ctx, logits, target, divisor: int):
+        logits, target = _f32(logits), _f32(target)
+        if target.shape != logits.shape:
+            raise ValueError(f"target {tuple(target.shape)} differs from logits {tuple(logits.shape)}")
+        loss = torch.empty(1, dtype=torch.float32, device=logits.device)
+        dl = torch.empty_like(logits)
+        runtime.train_bce_sum(logits.data_ptr(), target.data_ptr(), dl.data_ptr(), loss.data_ptr(), logits.numel(), int(divisor),
+                              _stream(logits))
+        ctx.save_for_backward(dl)
+        return loss[0]
+
+    @staticmethod
+    def backward(ctx, g):
+        (dl,) = ctx.saved_tensors
+        return dl * g, None, None
+
+
 class FusedAdam:
     """torch.optim.Adam semantics (L2 weight decay added to the gradient, bias-corrected) in ONE launch over all
     parameters; `groups` = [(params, weight_decay), ...] like the two groups of train.py:97-123."""

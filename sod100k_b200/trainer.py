@@ -121,3 +121,92 @@ class Trainer:
         self.flat.all_reduce_mean(self.group)
         self.opt.step()
         return loss.detach()
+
+
+class CSFSchedule:
+    """solver.train's bookkeeping (CSF+Res2Net/solver.py:81-127): `aveGrad` counts micro-steps across epochs and every iter_size-th
+    one takes an Adam step; after epoch e in lr_decay_epochs, lr is multiplied by 0.1 and a new Adam (zero moments, step 0) is built.
+    The epoch-start net.zero_grad() discards a partial accumulation but keeps the count, so an epoch's first Adam step can sum fewer
+    than iter_size micro-steps."""
+
+    def __init__(self, iter_size: int, lr: float, lr_decay_epochs=(15,)):
+        if int(iter_size) < 1:
+            raise ValueError(f"iter_size must be >= 1, got {iter_size}")
+        self.iter_size, self.lr, self.decay = int(iter_size), float(lr), frozenset(int(e) for e in lr_decay_epochs)
+        self.count = 0
+
+    def micro_step(self) -> bool:
+        """Count one micro-step; True when it ends with an Adam step."""
+        self.count += 1
+        if self.count % self.iter_size == 0:
+            self.count = 0
+            return True
+        return False
+
+    def epoch_end(self, epoch: int) -> bool:
+        """True when epoch `epoch` decays lr (and the optimiser is rebuilt)."""
+        if epoch in self.decay:
+            self.lr *= 0.1
+            return True
+        return False
+
+
+class CSFTrainer:
+    """CSF+Res2Net/solver.py:train's step on the device: forward on the module's training path in eval mode (frozen BatchNorm, as
+    solver.py:49 keeps the net), BCE summed over the batch / (iter_size * batch_size) (BceSumFn, no host sync), backward into one flat
+    gradient bucket (FlatGrads), and every iter_size-th micro-step one FusedAdam launch (torch.optim.Adam with L2 weight decay, betas
+    (0.9, 0.999), eps 1e-8) over the trainable parameters, then a zeroed bucket.  Training runs in fp32 whatever set_precision says.
+
+        trainer = CSFTrainer(net, iter_size=10)
+        for epoch in range(epochs):
+            trainer.epoch_begin()
+            rng = random.Random(base_seed)                    # the reference's per-epoch worker seed
+            for i in torch.randperm(len(ds)).tolist():
+                loss = trainer.step(*ds.csf_train_batch([i], rng))
+            trainer.epoch_end(epoch)
+
+    Gradients live in the bucket: a net.zero_grad() (or anything else that replaces p.grad) makes the next step raise EngineError."""
+
+    def __init__(self, net, lr: float = 5e-5, weight_decay: float = 5e-4, iter_size: int = 10, lr_decay_epochs=(15,),
+                 batch_size: int = 1):
+        if int(batch_size) < 1:
+            raise ValueError(f"batch_size must be >= 1, got {batch_size}")
+        self.net = net
+        self.schedule = CSFSchedule(iter_size, lr, lr_decay_epochs)
+        self.divisor = self.schedule.iter_size * int(batch_size)
+        self.weight_decay = float(weight_decay)
+        self.flat = FlatGrads(net.parameters())
+        self.opt = self._adam()
+
+    def _adam(self) -> T.FusedAdam:
+        return T.FusedAdam([(self.flat.params, self.weight_decay)], lr=self.schedule.lr, betas=(0.9, 0.999), eps=1e-8)
+
+    def _check_bucket(self):
+        if not self.flat.intact():
+            raise T.runtime.EngineError("gradient views were replaced (net.zero_grad()?); the flat bucket is stale — use "
+                                        "CSFTrainer.epoch_begin() to discard gradients")
+
+    def epoch_begin(self):
+        """The epoch-start net.zero_grad(): discards a partial accumulation, keeps the micro-step count."""
+        self._check_bucket()
+        self.flat.zero()
+
+    def step(self, x: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
+        """One micro-step on CUDA fp32 x [N,3,H,W] and target [N,1,H,W]; returns its loss (sum-BCE / divisor) as a device tensor."""
+        self._check_bucket()
+        if self.net.training:                          # eval() walks every sub-module: about 1 ms of host time a step
+            self.net.eval()
+        with torch.enable_grad():
+            out = self.net(x)
+            loss = T.BceSumFn.apply(out, target, self.divisor)
+            loss.backward()
+        self._check_bucket()
+        if self.schedule.micro_step():
+            self.opt.step()
+            self.flat.zero()
+        return loss.detach()
+
+    def epoch_end(self, epoch: int):
+        """Learning-rate decay after epoch `epoch` in lr_decay_epochs, with fresh Adam state."""
+        if self.schedule.epoch_end(epoch):
+            self.opt = self._adam()
