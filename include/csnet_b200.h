@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define CSNET_ABI_VERSION 12
+#define CSNET_ABI_VERSION 13
 
 enum { CSNET_F32 = 0, CSNET_F16 = 1, CSNET_BF16 = 2 };
 
@@ -313,7 +313,7 @@ int csnet_salmetric_csf_u8(const float* logits, int32_t N, int32_t H, int32_t W,
                            uint8_t* y_packed, uint32_t* hist_all, uint32_t* hist_pos, unsigned long long* abs_sum, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * Training primitives (fp32 planar NCHW device tensors).  The reference trains through torch autograd
+ * Training primitives (fp32 planar NCHW device tensors; the _bf16 calls below store activations in bf16).  The reference trains through torch autograd
  * (CSNet_training/train.py:203-216); train-mode BatchNorm makes the reference MODULE the closed unit, so the
  * boundary is one call per module piece.  sod100k_b200/train_ops.py wraps them in torch.autograd.Function s.
  * All return 0 / CSNET_E_*; csnet_train_last_error() holds the message.
@@ -322,7 +322,7 @@ int csnet_salmetric_csf_u8(const float* logits, int32_t N, int32_t H, int32_t W,
 /* One path of a raw (pre-BN) conv mix, device pointers resolved.  Same semantics as csnet_path_desc; `w` is the
  * path's weight in kernel layout [cin][ksize*ksize][cout] (fp32), NULL for resample-add paths (ksize == 0). */
 typedef struct {
-  const void* src;        /* fp32 [N, C, H, W] */
+  const void* src;        /* [N, C, H, W]: fp32 for the calls above, the call's source dtype for the _bf16 calls */
   const float* w;
   int32_t C, H, W;
   int32_t c0, cin;
@@ -386,6 +386,42 @@ int csnet_train_bce_sum(const float* logits, const float* target, float* dlogits
  * {float* p; const float* g; float* m; float* v; int32 n; float weight_decay} (40 bytes each). */
 int csnet_train_adam(const void* chunk_table_device, int32_t n_chunks, float lr, float beta1, float beta2, float eps, int32_t step,
                      float grad_scale, void* stream);
+
+/* ---- bf16 activation storage (sod100k_b200/train_ops.py picks these when the step stores bf16) ---------------------------------
+ * The same operations as the fp32 calls above, on bf16 planar NCHW activations and activation gradients (pointers are void*).
+ * Weights, weight gradients, BatchNorm mean / var / gamma / beta / slope and their gradients, and the per-image channel means stay
+ * fp32; every kernel accumulates in fp32 and rounds each bf16 store to nearest even; reductions keep the fp32 calls' order (no
+ * floating-point atomics: the same bits on every run).  Where a call can mix types, a dtype argument (CSNET_BF16 or CSNET_F32)
+ * names each side, and at least one side is bf16: the stem reads the fp32 network input, cls_layer writes fp32 logits.
+ * A shape the register-tiled kernels do not take (a stride-2 or pooled conv path not materialised by _pool_fwd_bf16, rows wider
+ * than 1024 pixels, mixed kernel sizes in one mix, a 1x1 mix with over 96 KiB of weights) returns CSNET_E_UNSUPPORTED; nothing is
+ * computed in fp32 behind the caller. */
+int csnet_train_bn_stats_bf16(const void* z, int32_t N, int32_t C, int32_t HW, float* mean, float* var, void* stream);
+int csnet_train_bn_prelu_fwd_bf16(const void* z, void* y, int32_t N, int32_t C, int32_t HW, const float* mean, const float* var,
+                                  const float* gamma, const float* beta, const float* slope, float eps, float* gap, void* stream);
+int csnet_train_bn_prelu_bwd_bf16(const void* z, const void* dy, void* dz, int32_t N, int32_t C, int32_t HW, const float* mean,
+                                  const float* var, const float* gamma, const float* beta, const float* slope, float eps,
+                                  float* dgamma, float* dbeta, float* dslope, int32_t frozen, void* stream);
+int csnet_train_dw_conv_bf16(const void* x, const float* w, void* y, int32_t N, int32_t C, int32_t H, int32_t W, float scale,
+                             int32_t transposed, void* stream);
+int csnet_train_dw_wgrad_bf16(const void* x, const void* dy, float* dw, int32_t N, int32_t C, int32_t H, int32_t W, float scale,
+                              void* stream);
+int csnet_train_dw_bwd_bf16(const void* x, const void* dy, const float* w, void* dx, float* dw, int32_t N, int32_t C, int32_t H,
+                            int32_t W, float scale, void* stream);
+/* every path's src has src_dtype; dst has dst_dtype */
+int csnet_train_mix_fwd_bf16(void* dst, int32_t dst_dtype, int32_t N, int32_t C, int32_t H, int32_t W, const csnet_train_path* paths,
+                             int32_t n_paths, int32_t src_dtype, void* stream);
+/* conv paths: ddst / dsrc of the given dtypes; resample paths: both bf16 */
+int csnet_train_mix_dgrad_bf16(const void* ddst, int32_t ddst_dtype, int32_t N, int32_t C, int32_t H, int32_t W,
+                               const csnet_train_path* path, void* dsrc, int32_t dsrc_dtype, void* stream);
+/* path.src has src_dtype, ddst has ddst_dtype; dw is fp32 */
+int csnet_train_mix_wgrad_bf16(const void* ddst, int32_t ddst_dtype, int32_t N, int32_t C, int32_t H, int32_t W,
+                               const csnet_train_path* path, float* dw, int32_t src_dtype, void* stream);
+/* the pooled copy of a bf16 source is bf16 */
+int csnet_train_pool_fwd_bf16(const void* src, int32_t N, int32_t Cs, int32_t c0, int32_t cin, int32_t Hs, int32_t Ws, int32_t pre_avg,
+                              int32_t pool, void* dst, uint8_t* idx, void* stream);
+int csnet_train_pool_bwd_bf16(const void* dpool, const uint8_t* idx, int32_t N, int32_t cin, int32_t Hs, int32_t Ws, int32_t pre_avg,
+                              int32_t pool, void* dsrc, void* stream);
 
 /* ---- CSF+Res2Net head training (fp32; sod100k_b200/modular_r.py wraps them) ---------------------------------------------------
  * Convolutions as an fp32 FMA implicit GEMM (csrc/gemm_f32.cuh).  One segment is one stride-1 convolution of a channel slice of

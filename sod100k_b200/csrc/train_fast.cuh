@@ -1,10 +1,11 @@
-// train_fast.cuh — register-tiled fp32 kernels of the training step (CSNet_training/train.py:203-216: F.conv2d forward, its data
+// train_fast.cuh — the fp32 __global__s of the register-tiled training kernels (CSNet_training/train.py:203-216: F.conv2d forward, its data
 // and weight gradients as autograd computes them; model/csnet.py:664-726 for the paths of a gOctaveConv).
 //
 // Everything here is DENSE: stride 1, same spatial size in and out, zero padding pad = dil * (k / 2).  The down-sampling a path
 // may carry (2x2 average of a stride-2 conv, max-pool of a high -> low path) is materialised once by pool_fwd_kernel (with the
 // arg-max, so the backward routes exactly like max_pool2d: first maximum in row-major order), so the three convolution kernels
-// never see it.  fp32 storage and fp32 FMA (the parity configuration: gradients within 1e-3 of autograd); the FP32 pipe is the
+// never see it.  The per-thread bodies live in train_body.cuh, templated on the activation type; these are their fp32 instances
+// (train_bf16.cu holds the bf16-storage ones).  fp32 storage and fp32 FMA (the parity configuration: gradients within 1e-3 of autograd); the FP32 pipe is the
 // roofline of these kernels, so each thread owns a 4 px x 16 channel (forward / dgrad) or 4 x 4 (x 3 taps) (wgrad) register tile
 // and reads its operands from shared memory as 16-byte vectors.
 //
@@ -20,517 +21,32 @@
 //                         the rows; the backward produces dx and the dw partials in one pass over dy.
 //   pool_fwd / pool2_fwd / pool_bwd(4), resample_bwd_kernel<UP>   the pooling a path carries (with arg-max) and the bilinear adjoint.
 #pragma once
-#include <cuda_runtime.h>
-
-#include <cstdint>
+#include "train_body.cuh"
 
 namespace csnet {
 namespace tf {
 
-constexpr int kT = 256;
-constexpr int kCoT = 16;            // output channels per thread (forward / dgrad)
-constexpr int kMaxConv = 5;         // conv paths of one mix (MSBlock: five dilations)
-constexpr int kMaxRs = 3;
-
-struct ConvPath {
-  const float* src;                 // [N][Cs][H][W]
-  const float* w;                   // [cin][k*k][cout]  (forward layout; dgrad reads it transposed)
-  int32_t Cs, c0, cin, cout0, cout, dil;
-  int32_t halo, Wp, rows, chunk;    // staged tile: rows = R + 2 halo rows of Wp floats (image column x at x + hp), chunk = ci per stage
-  int32_t hp;                       // column pad (multiple of 4, >= halo)
-};
-
-struct RsPath {
-  const float* src;                 // [N][Cs][Hs][Ws]
-  int32_t Cs, c0, Hs, Ws, up, cout0, cout;
-};
-
-struct ConvArgs {
-  float* dst;
-  int32_t N, C, H, W;               // destination
-  int32_t ksize, transposed;
-  int32_t n_conv, n_rs;
-  int32_t R, ipb, quads;            // tile: ipb images x R rows; quads = ceil(W / 4)
-  int32_t vec;                      // W % 4 == 0: 16-byte global loads / stores
-  int32_t tile_floats;              // shared-memory floats of the input tile region
-  ConvPath p[kMaxConv];
-  RsPath rs[kMaxRs];
-};
-
-__device__ __forceinline__ void cp_async16(float* dst_smem, const float* src, bool valid) {
-  const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst_smem);
-  const int sz = valid ? 16 : 0;                                   // src-size 0: the 16 bytes are zero-filled
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(d), "l"(src), "r"(sz) : "memory");
-}
-
-__device__ __forceinline__ void bilin(int H, int W, int up, int oy, int ox, int& o00, int& o01, int& o10, int& o11, float& w00,
-                                      float& w01, float& w10, float& w11) {
-  const float inv = 1.f / (float)up;
-  float sy = ((float)oy + 0.5f) * inv - 0.5f, sx = ((float)ox + 0.5f) * inv - 0.5f;
-  sy = sy < 0.f ? 0.f : sy; sx = sx < 0.f ? 0.f : sx;
-  const int y0 = (int)sy, x0 = (int)sx, y1 = y0 + (y0 < H - 1 ? 1 : 0), x1 = x0 + (x0 < W - 1 ? 1 : 0);
-  const float ly = sy - (float)y0, lx = sx - (float)x0;
-  o00 = y0 * W + x0; o01 = y0 * W + x1; o10 = y1 * W + x0; o11 = y1 * W + x1;
-  w00 = (1.f - ly) * (1.f - lx); w01 = (1.f - ly) * lx; w10 = ly * (1.f - lx); w11 = ly * lx;
-}
-
-// KS: 3 with dil == 1 (vector shared-memory reads); 0: any ksize / dilation (scalar reads; the MSBlock's dilated paths).  1x1 mixes run
-// on conv1x1_kernel below.
 template <int KS>
 __global__ void __launch_bounds__(kT, 2) conv_fwd_kernel(const __grid_constant__ ConvArgs A) {
   extern __shared__ __align__(16) float smem[];
-  float* tile = smem;                                   // [chunk][ipb][rows][Wp]
-  float* wsm = smem + A.tile_floats;                    // [chunk][kk][kCoT]
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int kk = A.ksize * A.ksize, H = A.H, W = A.W, R = A.R, ipb = A.ipb;
-  const int bands = (H + R - 1) / R;
-  const int n0 = (blockIdx.x / bands) * ipb, r0 = (blockIdx.x % bands) * R;
-  const int tasks = ipb * R * A.quads;
-  const bool live = tid < tasks;
-  const int ti = live ? tid / (R * A.quads) : 0, tr = live ? (tid / A.quads) % R : 0, tq = live ? tid % A.quads : 0;
-  const int n = n0 + ti, y = r0 + tr, x0 = 4 * tq;
-  const bool ok = live && n < A.N && y < H;
-  const size_t plane = (size_t)H * W;
-
-  // one path whose channels fit one stage: the input tile is staged once and reused by every output-channel group
-  const bool once = A.n_conv == 1 && A.p[0].chunk >= A.p[0].cin;
-  for (int cg = 0; cg * kCoT < A.C; ++cg) {
-    const int cb = cg * kCoT;
-    float acc[kCoT][4];
-#pragma unroll
-    for (int c = 0; c < kCoT; ++c) { acc[c][0] = acc[c][1] = acc[c][2] = acc[c][3] = 0.f; }
-    for (int pi = 0; pi < A.n_conv; ++pi) {
-      const ConvPath& P = A.p[pi];
-      if (P.cout0 >= cb + kCoT || P.cout0 + P.cout <= cb) continue;
-      const int trows = ipb * P.rows;                                      // staged rows per input channel
-      for (int ci0 = 0; ci0 < P.cin; ci0 += P.chunk) {
-        const int nc = P.cin - ci0 < P.chunk ? P.cin - ci0 : P.chunk;
-        __syncthreads();
-        // ---- stage the input tile: one warp per (channel, image, row), zero outside the image -------------------------------
-        for (int rr = warp; rr < ((once && cg > 0) ? 0 : nc * trows); rr += kT / 32) {
-          const int c = rr / trows, ir = rr - c * trows, i = ir / P.rows, row = ir - i * P.rows;
-          const int gy = r0 + row - P.halo, gn = n0 + i;
-          float* d = tile + (size_t)rr * P.Wp;
-          const bool inside = gy >= 0 && gy < H && gn < A.N;
-          const float* s = P.src + (((size_t)gn * P.Cs + P.c0 + ci0 + c) * H + (inside ? gy : 0)) * W;
-          if (A.vec) {
-            for (int v = lane; v * 4 < P.Wp; v += 32) {
-              const int xx = v * 4 - P.hp;
-              const bool ld = inside && xx >= 0 && xx < W;
-              cp_async16(d + v * 4, ld ? s + xx : P.src, ld);             // asynchronous: every row of the stage is in flight at once
-            }
-          } else {
-            for (int v = lane; v < P.Wp; v += 32) {
-              const int xx = v - P.hp;
-              d[v] = (inside && xx >= 0 && xx < W) ? __ldg(s + xx) : 0.f;
-            }
-          }
-        }
-        asm volatile("cp.async.commit_group;\n" ::: "memory");
-        // ---- stage the weights of this (channel chunk, output-channel group); zero outside the path's slice ------------------
-        for (int i = tid; i < nc * kk * kCoT; i += kT) {
-          const int c = i / (kk * kCoT), t = (i / kCoT) % kk, co = cb + (i % kCoT) - P.cout0;
-          float v = 0.f;
-          if (co >= 0 && co < P.cout)
-            v = A.transposed ? __ldg(P.w + ((size_t)co * kk + (kk - 1 - t)) * P.cin + ci0 + c)       // dgrad: w'[ci'=co][flip t][co'=ci]
-                             : __ldg(P.w + ((size_t)(ci0 + c) * kk + t) * P.cout + co);
-          wsm[i] = v;
-        }
-        asm volatile("cp.async.wait_group 0;\n" ::: "memory");
-        __syncthreads();
-        if (!live) continue;
-        // ---- accumulate ---------------------------------------------------------------------------------------------------
-        const float* tb = tile + ((size_t)ti * P.rows + tr) * P.Wp + x0 + P.hp;          // tap (0, 0) of a 1x1; (ky, kx) offsets below
-        for (int c = 0; c < nc; ++c) {
-          const float* tc = tb + (size_t)c * trows * P.Wp;
-          const float* wc = wsm + c * kk * kCoT;
-          if (KS == 3) {
-#pragma unroll
-            for (int ky = 0; ky < 3; ++ky) {
-              const float* tr_ = tc + (ky * P.Wp) - 4;                              // halo == 1: rows y-1..y+1 are tile rows tr..tr+2
-              const float l = tr_[3];
-              const float4 m = *reinterpret_cast<const float4*>(tr_ + 4);
-              const float r = tr_[8];
-              const float in[6] = {l, m.x, m.y, m.z, m.w, r};
-#pragma unroll
-              for (int kx = 0; kx < 3; ++kx) {
-#pragma unroll
-                for (int q = 0; q < kCoT / 4; ++q) {
-                  const float4 w4 = *reinterpret_cast<const float4*>(wc + (ky * 3 + kx) * kCoT + 4 * q);
-                  const float wv[4] = {w4.x, w4.y, w4.z, w4.w};
-#pragma unroll
-                  for (int j = 0; j < 4; ++j) {
-#pragma unroll
-                    for (int px = 0; px < 4; ++px) acc[4 * q + j][px] = fmaf(in[px + kx], wv[j], acc[4 * q + j][px]);
-                  }
-                }
-              }
-            }
-          } else {
-            const int ks = A.ksize, hk = ks / 2;
-            for (int ky = 0; ky < ks; ++ky) {
-              for (int kx = 0; kx < ks; ++kx) {
-                const float* tp = tc + ((ky - hk) * P.dil + P.halo) * P.Wp + (kx - hk) * P.dil;
-                const float in[4] = {tp[0], tp[1], tp[2], tp[3]};
-#pragma unroll
-                for (int q = 0; q < kCoT / 4; ++q) {
-                  const float4 w4 = *reinterpret_cast<const float4*>(wc + (ky * ks + kx) * kCoT + 4 * q);
-                  const float wv[4] = {w4.x, w4.y, w4.z, w4.w};
-#pragma unroll
-                  for (int j = 0; j < 4; ++j) {
-#pragma unroll
-                    for (int px = 0; px < 4; ++px) acc[4 * q + j][px] = fmaf(in[px], wv[j], acc[4 * q + j][px]);
-                  }
-                }
-              }
-            }
-          }
-        }
-      }
-    }
-    if (!ok) continue;
-    // ---- resample-add paths (bilinear x up of a low-resolution tensor; align_corners=False, F.interpolate semantics) ------------
-    for (int ri = 0; ri < A.n_rs; ++ri) {
-      const RsPath& Q = A.rs[ri];
-      if (Q.cout0 >= cb + kCoT || Q.cout0 + Q.cout <= cb) continue;
-      const size_t lp = (size_t)Q.Hs * Q.Ws;
-#pragma unroll
-      for (int px = 0; px < 4; ++px) {
-        if (x0 + px >= W) continue;
-        int o00, o01, o10, o11;
-        float w00, w01, w10, w11;
-        bilin(Q.Hs, Q.Ws, Q.up, y, x0 + px, o00, o01, o10, o11, w00, w01, w10, w11);
-#pragma unroll
-        for (int c = 0; c < kCoT; ++c) {
-          const int co = cb + c - Q.cout0;
-          if (co < 0 || co >= Q.cout) continue;
-          const float* s = Q.src + ((size_t)n * Q.Cs + Q.c0 + co) * lp;
-          acc[c][px] += w00 * __ldg(s + o00) + w01 * __ldg(s + o01) + w10 * __ldg(s + o10) + w11 * __ldg(s + o11);
-        }
-      }
-    }
-    float* o = A.dst + (((size_t)n * A.C + cb) * H + y) * W + x0;
-#pragma unroll
-    for (int c = 0; c < kCoT; ++c) {
-      if (cb + c >= A.C) break;
-      if (A.vec) {
-        *reinterpret_cast<float4*>(o + (size_t)c * plane) = make_float4(acc[c][0], acc[c][1], acc[c][2], acc[c][3]);
-      } else {
-#pragma unroll
-        for (int px = 0; px < 4; ++px)
-          if (x0 + px < W) o[(size_t)c * plane + px] = acc[c][px];
-      }
-    }
-  }
+  conv_fwd_body<KS, float, float>(A, smem);
 }
 
-// ---- 1x1 convolution mix, direct form ------------------------------------------------------------------------------------------------
-// A 1x1 path needs each input element in exactly one thread (the one that owns its pixel, for every output channel), so the inputs go
-// global -> registers as 16-byte loads (re-reads for a second output-channel group hit L1) and only the weights live in shared
-// memory: no tile staging, no barriers after the prologue.  Also runs a mix that has only resample-add paths (n_conv == 0).
-struct C1Path {
-  const float* src;
-  const float* w;
-  int32_t Cs, c0, cin, cout0, cout, woff;          // woff: first weight row of this path in shared memory
-};
-
-struct C1Args {
-  float* dst;
-  int32_t N, C, H, W, quads, vec, transposed, n_conv, n_rs, Cpad, wrows;
-  C1Path p[kMaxConv];
-  RsPath rs[kMaxRs];
-};
-
-template <int CT, int PX, bool VEC, int U = 6>           // U: input channels loaded ahead of their FMAs (memory-level parallelism)
-__device__ __forceinline__ void c1_group(const C1Args& A, const float* wsm, int cb, int n, int y, int x0) {
-  const int H = A.H, W = A.W;
-  const size_t plane = (size_t)H * W;
-  float acc[CT][PX];
-#pragma unroll
-  for (int c = 0; c < CT; ++c)
-#pragma unroll
-    for (int px = 0; px < PX; ++px) acc[c][px] = 0.f;
-  for (int pi = 0; pi < A.n_conv; ++pi) {
-    const C1Path& P = A.p[pi];
-    if (P.cout0 >= cb + CT || P.cout0 + P.cout <= cb) continue;
-    const float* s = P.src + (((size_t)n * P.Cs + P.c0) * H + y) * W + x0;
-    const float* wr = wsm + (size_t)P.woff * A.Cpad + cb;
-    for (int ci0 = 0; ci0 < P.cin; ci0 += U) {
-      float v[U][PX];
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const float* q = s + (size_t)(ci0 + u) * plane;
-        const bool on = ci0 + u < P.cin;
-        if (VEC) {
-          if (PX == 4) {
-            float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (on) t = __ldg(reinterpret_cast<const float4*>(q));
-            v[u][0] = t.x; v[u][1] = t.y; v[u][PX - 2] = t.z; v[u][PX - 1] = t.w;
-          } else {
-            float2 t = make_float2(0.f, 0.f);
-            if (on) t = __ldg(reinterpret_cast<const float2*>(q));
-            v[u][0] = t.x; v[u][1] = t.y;
-          }
-        } else {
-#pragma unroll
-          for (int px = 0; px < PX; ++px) v[u][px] = (on && x0 + px < W) ? __ldg(q + px) : 0.f;
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        if (ci0 + u >= P.cin) break;
-#pragma unroll
-        for (int q4 = 0; q4 < CT / 4; ++q4) {
-          const float4 w4 = *reinterpret_cast<const float4*>(wr + (size_t)(ci0 + u) * A.Cpad + 4 * q4);
-          const float wv[4] = {w4.x, w4.y, w4.z, w4.w};
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-#pragma unroll
-            for (int px = 0; px < PX; ++px) acc[4 * q4 + j][px] = fmaf(v[u][px], wv[j], acc[4 * q4 + j][px]);
-        }
-      }
-    }
-  }
-  for (int ri = 0; ri < A.n_rs; ++ri) {
-    const RsPath& Q = A.rs[ri];
-    if (Q.cout0 >= cb + CT || Q.cout0 + Q.cout <= cb) continue;
-    const size_t lp = (size_t)Q.Hs * Q.Ws;
-#pragma unroll
-    for (int px = 0; px < PX; ++px) {
-      if (x0 + px >= W) continue;
-      int o00, o01, o10, o11;
-      float w00, w01, w10, w11;
-      bilin(Q.Hs, Q.Ws, Q.up, y, x0 + px, o00, o01, o10, o11, w00, w01, w10, w11);
-#pragma unroll
-      for (int c = 0; c < CT; ++c) {
-        const int co = cb + c - Q.cout0;
-        if (co < 0 || co >= Q.cout) continue;
-        const float* sp = Q.src + ((size_t)n * Q.Cs + Q.c0 + co) * lp;
-        acc[c][px] += w00 * __ldg(sp + o00) + w01 * __ldg(sp + o01) + w10 * __ldg(sp + o10) + w11 * __ldg(sp + o11);
-      }
-    }
-  }
-  float* o = A.dst + (((size_t)n * A.C + cb) * H + y) * W + x0;
-#pragma unroll
-  for (int c = 0; c < CT; ++c) {
-    if (cb + c >= A.C) break;
-    if (VEC) {
-      if (PX == 4) *reinterpret_cast<float4*>(o + (size_t)c * plane) = make_float4(acc[c][0], acc[c][1], acc[c][PX - 2], acc[c][PX - 1]);
-      else *reinterpret_cast<float2*>(o + (size_t)c * plane) = make_float2(acc[c][0], acc[c][1]);
-    } else {
-#pragma unroll
-      for (int px = 0; px < PX; ++px)
-        if (x0 + px < W) o[(size_t)c * plane + px] = acc[c][px];
-    }
-  }
-}
-
-// PX == 4: 4 pixels x (16 | 8) channels per pass (<= 16 output channels: one pass over the input);  PX == 2: 2 pixels x (32 | 16 | 8)
-// channels (17..32 output channels in ONE pass).  quads = ceil(W / PX), vec = W % PX == 0.
 template <int PX, bool VEC>
 __global__ void __launch_bounds__(kT, 2) conv1x1_kernel(const __grid_constant__ C1Args A) {
   extern __shared__ __align__(16) float wsm[];                          // [wrows][Cpad]: every path's weights, zero outside its slice
-  for (int i = threadIdx.x; i < A.wrows * A.Cpad; i += kT) {
-    const int row = i / A.Cpad, col = i - row * A.Cpad;
-    float v = 0.f;
-    for (int pi = 0; pi < A.n_conv; ++pi) {
-      const C1Path& P = A.p[pi];
-      const int ci = row - P.woff, co = col - P.cout0;
-      if (ci >= 0 && ci < P.cin && co >= 0 && co < P.cout)
-        v = A.transposed ? __ldg(P.w + (size_t)co * P.cin + ci) : __ldg(P.w + (size_t)ci * P.cout + co);
-    }
-    wsm[i] = v;
-  }
-  __syncthreads();
-  const size_t task = (size_t)blockIdx.x * kT + threadIdx.x;
-  if (task >= (size_t)A.N * A.H * A.quads) return;
-  const int q = (int)(task % A.quads), y = (int)((task / A.quads) % A.H), n = (int)(task / ((size_t)A.quads * A.H));
-  for (int cb = 0; cb < A.C;) {
-    const int left = A.C - cb;
-    if (left <= 8) { c1_group<8, PX, VEC>(A, wsm, cb, n, y, PX * q); cb += 8; }
-    else if (PX == 4 || left <= 16) { c1_group<16, PX, VEC>(A, wsm, cb, n, y, PX * q); cb += 16; }
-    else { c1_group<32, PX, VEC>(A, wsm, cb, n, y, PX * q); cb += 32; }
-  }
+  conv1x1_body<PX, VEC, float, float>(A, wsm);
 }
 
-// narrow form: 8 output channels per pass and 8 channels of loads in flight, <= 85 registers so three CTAs fit an SM
 __global__ void __launch_bounds__(kT, 3) conv1x1_narrow_kernel(const __grid_constant__ C1Args A) {
   extern __shared__ __align__(16) float wsm[];
-  for (int i = threadIdx.x; i < A.wrows * A.Cpad; i += kT) {
-    const int row = i / A.Cpad, col = i - row * A.Cpad;
-    float v = 0.f;
-    for (int pi = 0; pi < A.n_conv; ++pi) {
-      const C1Path& P = A.p[pi];
-      const int ci = row - P.woff, co = col - P.cout0;
-      if (ci >= 0 && ci < P.cin && co >= 0 && co < P.cout)
-        v = A.transposed ? __ldg(P.w + (size_t)co * P.cin + ci) : __ldg(P.w + (size_t)ci * P.cout + co);
-    }
-    wsm[i] = v;
-  }
-  __syncthreads();
-  const size_t task = (size_t)blockIdx.x * kT + threadIdx.x;
-  if (task >= (size_t)A.N * A.H * A.quads) return;
-  const int q = (int)(task % A.quads), y = (int)((task / A.quads) % A.H), n = (int)(task / ((size_t)A.quads * A.H));
-  for (int cb = 0; cb < A.C; cb += 8) c1_group<8, 4, true, 8>(A, wsm, cb, n, y, 4 * q);
+  conv1x1_narrow_body<float, float>(A, wsm);
 }
 
-// ---- weight gradient ---------------------------------------------------------------------------------------------------------
-struct WgradArgs {
-  const float* in;                  // [N][Cs][H][W], channels [c0, c0 + cin)
-  const float* dd;                  // [N][Cd][H][W], channels [cout0, cout0 + cout)
-  float* part;                      // [grid][cin * kk * cout] partial sums (block order)
-  int32_t N, Cs, c0, cin, Cd, cout0, cout, H, W;
-  int32_t R, units;                 // row band; units = N * ceil(H / R)
-  int32_t Wp, quads;                // shared-memory pitch (W + 8, multiple of 4), quads = ceil(W / 4)
-  int32_t mt, nt, tiles, splits;    // thread tiles: mt = ceil(cin / 4) (x 3 tap rows for 3x3), nt = ceil(cout / 4); splits = pixel splits
-  int32_t tpad;                     // tiles per block (grid.y groups of tpad tiles): a multiple of 32, or a power of two < 32
-  int32_t cin4, cout4;              // channel counts rounded up to 4 (zero rows)
-  int32_t vec;
-  int32_t dil, hp;                  // dilation (KS == 0 form) and the column pad of the input tile (multiple of 4, >= dil)
-  int32_t cpi, cpd;                 // channel pitches of the two tiles in floats, == 4 (mod 32): the 4-channel thread tiles are interleaved
-                                    // (tile t owns channels t, t + M, t + 2M, t + 3M), so the lanes of a warp read distinct bank groups
-};
-
-// KS == 1: thread tile 4 ci x 4 co;  KS == 3: 4 ci x 4 co x the 3 taps of one kernel row (dil 1);  KS == 0: 3x3 with any dilation —
-// the input tile holds the three row bands r0 + (ky - 1) dil ... of a kernel row each, scalar shared-memory reads
 template <int KS>
 __global__ void __launch_bounds__(kT, 2) conv_wgrad_kernel(const __grid_constant__ WgradArgs A) {
   extern __shared__ __align__(16) float smem[];
-  constexpr int KX = KS == 1 ? 1 : 3, KY = KS == 1 ? 1 : 3;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int H = A.H, W = A.W, R = A.R, Wp = A.Wp, rows_in = KS == 0 ? 3 * R : R + (KS == 3 ? 2 : 0), hp = A.hp;
-  const int buf_floats = A.cin4 * A.cpi + A.cout4 * A.cpd;         // one stage: input tile [cin4][rows_in][Wp] (image column x at x + hp),
-  const int bands = (H + R - 1) / R;                               //            gradient tile [cout4][R][Wp] (column x at x)
-  // task of this thread: (pixel split, tile); tiles beyond A.tiles idle.  Threads of one warp share the split when tiles >= 32.
-  const int ltile = tid % A.tpad, split = tid / A.tpad, tile = blockIdx.y * A.tpad + ltile;
-  const bool active = tile < A.tiles && split < A.splits;
-  const int tm = active ? tile / A.nt : 0, tn = active ? tile % A.nt : 0;
-  const int ci_t = tm / KY, ky = tm % KY, co_t = tn, Mi = A.cin4 / 4, Mo = A.nt;     // channels ci_t + i * Mi, co_t + j * Mo
-  float acc[KX][4][4];
-#pragma unroll
-  for (int a = 0; a < KX; ++a)
-#pragma unroll
-    for (int b = 0; b < 4; ++b) acc[a][b][0] = acc[a][b][1] = acc[a][b][2] = acc[a][b][3] = 0.f;
-
-  // stage unit u into `base` with 16-byte cp.async (zero-filled outside the image / the channel range); rows that are not 16-byte
-  // multiples take the synchronous scalar route
-  auto stage = [&](int u, float* base) {
-    const int n = u / bands, r0 = (u % bands) * R;
-    float* tin = base;
-    float* tdd = base + (size_t)A.cin4 * A.cpi;
-    for (int rr = warp; rr < A.cin4 * rows_in; rr += kT / 32) {
-      const int c = rr / rows_in, row = rr - c * rows_in;
-      const int gy = KS == 0 ? r0 + row % R + (row / R - 1) * A.dil : r0 + row - (KS == 3 ? 1 : 0);
-      const bool inside = c < A.cin && gy >= 0 && gy < H && (KS != 0 || r0 + row % R < H);
-      const float* s = A.in + (((size_t)n * A.Cs + A.c0 + (inside ? c : 0)) * H + (inside ? gy : 0)) * W;
-      float* d = tin + (size_t)c * A.cpi + (size_t)row * Wp;
-      if (A.vec) {
-        for (int v = lane; v * 4 < Wp; v += 32) {
-          const int xx = v * 4 - hp;
-          const bool ld = inside && xx >= 0 && xx < W;
-          cp_async16(d + v * 4, ld ? s + xx : A.in, ld);
-        }
-      } else {
-        for (int v = lane; v < Wp; v += 32) {
-          const int xx = v - hp;
-          d[v] = (inside && xx >= 0 && xx < W) ? __ldg(s + xx) : 0.f;
-        }
-      }
-    }
-    for (int rr = warp; rr < A.cout4 * R; rr += kT / 32) {
-      const int c = rr / R, row = rr - c * R, gy = r0 + row;
-      const bool inside = c < A.cout && gy < H;
-      const float* s = A.dd + (((size_t)n * A.Cd + A.cout0 + (inside ? c : 0)) * H + (inside ? gy : 0)) * W;
-      float* d = tdd + (size_t)c * A.cpd + (size_t)row * Wp;
-      if (A.vec) {
-        for (int v = lane; v * 4 < Wp; v += 32) {
-          const int xx = v * 4;
-          const bool ld = inside && xx < W;
-          cp_async16(d + v * 4, ld ? s + xx : A.dd, ld);
-        }
-      } else {
-        for (int v = lane; v < Wp; v += 32) d[v] = (inside && v < W) ? __ldg(s + v) : 0.f;
-      }
-    }
-  };
-
-  // two stages in flight: unit u+grid is copied while unit u is consumed
-  int cur = 0;
-  if ((int)blockIdx.x < A.units) stage(blockIdx.x, smem);
-  asm volatile("cp.async.commit_group;\n" ::: "memory");
-  for (int u = blockIdx.x; u < A.units; u += gridDim.x, cur ^= 1) {
-    const int un = u + gridDim.x;
-    if (un < A.units) stage(un, smem + (size_t)(cur ^ 1) * buf_floats);
-    asm volatile("cp.async.commit_group;\n" ::: "memory");
-    asm volatile("cp.async.wait_group 1;\n" ::: "memory");
-    __syncthreads();
-    const float* tin = smem + (size_t)cur * buf_floats;
-    const float* tdd = tin + (size_t)A.cin4 * A.cpi;
-    if (active) {
-    const int nq = R * A.quads;
-    for (int q = split; q < nq; q += A.splits) {
-      const int row = q / A.quads, x0 = 4 * (q - row * A.quads);
-      float4 d4[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) d4[j] = *reinterpret_cast<const float4*>(tdd + (size_t)(co_t + j * Mo) * A.cpd + (size_t)row * Wp + x0);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const float* ip = tin + (size_t)(ci_t + i * Mi) * A.cpi + (size_t)(KS == 0 ? ky * R + row : row + ky) * Wp + x0 + hp;
-        if (KS == 0) {
-#pragma unroll
-          for (int kx = 0; kx < 3; ++kx) {
-            const float* tp = ip + (kx - 1) * A.dil;
-            const float i0 = tp[0], i1 = tp[1], i2 = tp[2], i3 = tp[3];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) acc[kx][i][j] += i0 * d4[j].x + i1 * d4[j].y + i2 * d4[j].z + i3 * d4[j].w;
-          }
-        } else if (KS == 1) {
-          const float4 v = *reinterpret_cast<const float4*>(ip);
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            acc[0][i][j] += v.x * d4[j].x + v.y * d4[j].y + v.z * d4[j].z + v.w * d4[j].w;
-        } else {
-          const float l = ip[-1];
-          const float4 m = *reinterpret_cast<const float4*>(ip);
-          const float r = ip[4];
-          const float in[6] = {l, m.x, m.y, m.z, m.w, r};
-#pragma unroll
-          for (int kx = 0; kx < 3; ++kx)
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              acc[kx][i][j] += in[kx] * d4[j].x + in[kx + 1] * d4[j].y + in[kx + 2] * d4[j].z + in[kx + 3] * d4[j].w;
-        }
-      }
-    }
-    }
-    __syncthreads();                                               // everyone is done with this stage before the next copy lands in it
-  }
-  asm volatile("cp.async.wait_group 0;\n" ::: "memory");
-  // ---- merge the pixel splits of the block in split order, write the block's partial ---------------------------------------------
-  __syncthreads();
-  float* red = smem;                                              // [splits][tpad][KX*16]
-  constexpr int TA = KX * 16;
-  if (active) {
-    float* o = red + ((size_t)split * A.tpad + ltile) * TA;
-#pragma unroll
-    for (int a = 0; a < KX; ++a)
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) o[(a * 4 + i) * 4 + j] = acc[a][i][j];
-  }
-  __syncthreads();
-  const int kk = KS == 1 ? 1 : 9;
-  float* out = A.part + (size_t)blockIdx.x * A.cin * kk * A.cout;
-  for (int e = tid; e < A.tpad * TA; e += kT) {
-    const int lt = e / TA, t = blockIdx.y * A.tpad + lt, r = e - lt * TA, a = r / 16, i = (r / 4) % 4, j = r % 4;
-    if (t >= A.tiles) continue;
-    const int tm2 = t / A.nt, tn2 = t % A.nt, ci = tm2 / KY + i * (A.cin4 / 4), ky2 = tm2 % KY, co = tn2 + j * A.nt;
-    if (ci >= A.cin || co >= A.cout) continue;
-    float s = 0.f;
-    for (int sp = 0; sp < A.splits; ++sp) s += red[((size_t)sp * A.tpad + lt) * TA + r];
-    out[((size_t)ci * kk + ky2 * KX + a) * A.cout + co] = s;
-  }
+  conv_wgrad_body<KS, float, float>(A, smem);
 }
 
 // out[e] = scale * sum over parts (in part order) of part[p][e]
@@ -546,356 +62,46 @@ __global__ void __launch_bounds__(kT) reduce_partials_kernel(const float* __rest
   out[e] = ((s0 + s1) + (s2 + s3)) * scale;
 }
 
-// ---- pooling prep (forward) and its routing (backward) ----------------------------------------------------------------------------
-// dst[n][ci][yc][xc] = max over pool x pool of (pre_avg ? 2x2 mean : value) of src channels [c0, c0 + cin); idx = position of the
-// FIRST maximum (row-major), as max_pool2d's backward uses it.
 __global__ void __launch_bounds__(kT) pool_fwd_kernel(const float* __restrict__ src, int N, int Cs, int c0, int cin, int Hs, int Ws, int pre_avg,
                                                       int pool, float* __restrict__ dst, uint8_t* __restrict__ idx) {
-  const int f = pre_avg ? 2 : 1, Hc = Hs / (f * pool), Wc = Ws / (f * pool);
-  const size_t i = (size_t)blockIdx.x * kT + threadIdx.x, total = (size_t)N * cin * Hc * Wc;
-  if (i >= total) return;
-  const int xc = (int)(i % Wc), yc = (int)((i / Wc) % Hc), c = (int)((i / ((size_t)Wc * Hc)) % cin), n = (int)(i / ((size_t)Wc * Hc * cin));
-  const float* s = src + ((size_t)n * Cs + c0 + c) * Hs * Ws;
-  float best = -INFINITY;
-  int bi = 0;
-  for (int py = 0; py < pool; ++py)
-    for (int px = 0; px < pool; ++px) {
-      const int ya = yc * pool + py, xa = xc * pool + px;
-      float v;
-      if (pre_avg) {
-        const float* b = s + (size_t)(2 * ya) * Ws + 2 * xa;
-        v = (((b[0] + b[1]) + b[Ws]) + b[Ws + 1]) * 0.25f;
-      } else {
-        v = s[(size_t)ya * Ws + xa];
-      }
-      if (v > best) { best = v; bi = py * pool + px; }
-    }
-  dst[i] = best;
-  if (idx) idx[i] = (uint8_t)bi;
+  pool_fwd_body(src, N, Cs, c0, cin, Hs, Ws, pre_avg, pool, dst, idx);
 }
 
-// pool == 2 without the average, Ws % 4 == 0: two outputs per thread from two 16-byte loads
 __global__ void __launch_bounds__(kT) pool2_fwd_kernel(const float* __restrict__ src, int N, int Cs, int c0, int cin, int Hs, int Ws,
                                                        float* __restrict__ dst, uint8_t* __restrict__ idx) {
-  const int Hc = Hs >> 1, Wc = Ws >> 1, W2 = Wc >> 1;
-  const unsigned t = blockIdx.x * kT + threadIdx.x, total = (unsigned)N * cin * Hc * W2;        // < 2^32: checked by the host
-  if (t >= total) return;
-  const int x2 = (int)(t % (unsigned)W2), yc = (int)((t / (unsigned)W2) % (unsigned)Hc);
-  const unsigned nc = t / ((unsigned)W2 * (unsigned)Hc);
-  const int c = (int)(nc % (unsigned)cin), n = (int)(nc / (unsigned)cin);
-  const float* s = src + (((size_t)n * Cs + c0 + c) * Hs + 2 * yc) * Ws + 4 * x2;
-  const float4 a = __ldg(reinterpret_cast<const float4*>(s)), b = __ldg(reinterpret_cast<const float4*>(s + Ws));
-  float m0 = a.x; int i0 = 0;
-  if (a.y > m0) { m0 = a.y; i0 = 1; }
-  if (b.x > m0) { m0 = b.x; i0 = 2; }
-  if (b.y > m0) { m0 = b.y; i0 = 3; }
-  float m1 = a.z; int i1 = 0;
-  if (a.w > m1) { m1 = a.w; i1 = 1; }
-  if (b.z > m1) { m1 = b.z; i1 = 2; }
-  if (b.w > m1) { m1 = b.w; i1 = 3; }
-  const size_t o = ((size_t)nc * Hc + yc) * Wc + 2 * x2;
-  *reinterpret_cast<float2*>(dst + o) = make_float2(m0, m1);
-  *reinterpret_cast<uchar2*>(idx + o) = make_uchar2((unsigned char)i0, (unsigned char)i1);
+  pool2_fwd_body(src, N, Cs, c0, cin, Hs, Ws, dst, idx);
 }
 
-// dsrc[n][ci][ys][xs] (exactly cin channels) from the gradient of the pooled tensor
 __global__ void __launch_bounds__(kT) pool_bwd_kernel(const float* __restrict__ dpool, const uint8_t* __restrict__ idx, int N, int cin, int Hs, int Ws,
                                                       int pre_avg, int pool, float* __restrict__ dsrc) {
-  const int f = pre_avg ? 2 : 1, Hc = Hs / (f * pool), Wc = Ws / (f * pool);
-  const size_t i = (size_t)blockIdx.x * kT + threadIdx.x, total = (size_t)N * cin * Hs * Ws;
-  if (i >= total) return;
-  const int xs = (int)(i % Ws), ys = (int)((i / Ws) % Hs);
-  const size_t nc = i / ((size_t)Ws * Hs);
-  const int ya = ys / f, xa = xs / f, yc = ya / pool, xc = xa / pool;
-  float g = 0.f;
-  if (yc < Hc && xc < Wc) {
-    const size_t j = (nc * Hc + yc) * Wc + xc;
-    const bool hit = pool == 1 || (int)idx[j] == (ya - yc * pool) * pool + (xa - xc * pool);
-    if (hit) g = dpool[j] * (pre_avg ? 0.25f : 1.f);
-  }
-  dsrc[i] = g;
+  pool_bwd_body(dpool, idx, N, cin, Hs, Ws, pre_avg, pool, dsrc);
 }
 
-// four consecutive source pixels per thread (Ws % 4 == 0)
 __global__ void __launch_bounds__(kT) pool_bwd4_kernel(const float* __restrict__ dpool, const uint8_t* __restrict__ idx, int N, int cin, int Hs, int Ws,
                                                        int pre_avg, int pool, float* __restrict__ dsrc) {
-  const int f = pre_avg ? 2 : 1, Hc = Hs / (f * pool), Wc = Ws / (f * pool), W4 = Ws >> 2;
-  const unsigned t = blockIdx.x * kT + threadIdx.x, total = (unsigned)N * cin * Hs * W4;     // < 2^32: checked by the host
-  if (t >= total) return;
-  const int x4 = (int)(t % (unsigned)W4), ys = (int)((t / (unsigned)W4) % (unsigned)Hs);
-  const size_t nc = t / ((unsigned)W4 * (unsigned)Hs);
-  const int ya = ys / f, yc = ya / pool;
-  float g[4];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const int xs = 4 * x4 + j, xa = xs / f, xc = xa / pool;
-    g[j] = 0.f;
-    if (yc < Hc && xc < Wc) {
-      const size_t k = (nc * Hc + yc) * Wc + xc;
-      const bool hit = pool == 1 || (int)__ldg(idx + k) == (ya - yc * pool) * pool + (xa - xc * pool);
-      if (hit) g[j] = __ldg(dpool + k) * (pre_avg ? 0.25f : 1.f);
-    }
-  }
-  *reinterpret_cast<float4*>(dsrc + (nc * Hs + ys) * Ws + 4 * x4) = make_float4(g[0], g[1], g[2], g[3]);
+  pool_bwd4_body(dpool, idx, N, cin, Hs, Ws, pre_avg, pool, dsrc);
 }
 
-// adjoint of the bilinear x UP resample (align_corners=False, source index clamped at 0): dsrc[n][c][ys][xs] for c < cin gathers the
-// (2 UP)^2 destination pixels that can feed it — rows UP ys - UP/2 ... UP ys + 3 UP/2 - 1, which also covers the clamped borders —
-// with separable weights computed once per thread.
 template <int UP>
 __global__ void __launch_bounds__(kT) resample_bwd_kernel(const float* __restrict__ ddst, int N, int C, int H, int W, int cout0, int cin, int Hs, int Ws,
                                                           float* __restrict__ dsrc) {
-  const unsigned t = blockIdx.x * kT + threadIdx.x, total = (unsigned)N * cin * Hs * Ws;         // < 2^32: checked by the host
-  if (t >= total) return;
-  const int xs = (int)(t % (unsigned)Ws), ys = (int)((t / (unsigned)Ws) % (unsigned)Hs);
-  const unsigned ncq = t / ((unsigned)Ws * (unsigned)Hs);
-  const int c = (int)(ncq % (unsigned)cin), n = (int)(ncq / (unsigned)cin);
-  constexpr float inv = 1.f / (float)UP;
-  constexpr int K = 2 * UP;
-  float wy[K], wx[K];
-  const int yb = ys * UP - UP / 2, xb = xs * UP - UP / 2;
-#pragma unroll
-  for (int k = 0; k < K; ++k) {
-    wy[k] = 0.f; wx[k] = 0.f;
-    const int oy = yb + k, ox = xb + k;
-    if (oy >= 0 && oy < H) {
-      float sy = ((float)oy + 0.5f) * inv - 0.5f;
-      sy = sy < 0.f ? 0.f : sy;
-      const int y0 = (int)sy, y1 = y0 + (y0 < Hs - 1 ? 1 : 0);
-      const float ly = sy - (float)y0;
-      wy[k] = (y0 == ys ? 1.f - ly : 0.f) + (y1 == ys ? ly : 0.f);
-    }
-    if (ox >= 0 && ox < W) {
-      float sx = ((float)ox + 0.5f) * inv - 0.5f;
-      sx = sx < 0.f ? 0.f : sx;
-      const int x0 = (int)sx, x1 = x0 + (x0 < Ws - 1 ? 1 : 0);
-      const float lx = sx - (float)x0;
-      wx[k] = (x0 == xs ? 1.f - lx : 0.f) + (x1 == xs ? lx : 0.f);
-    }
-  }
-  const float* d = ddst + ((size_t)n * C + cout0 + c) * H * W;
-  float g = 0.f;
-#pragma unroll
-  for (int ky = 0; ky < K; ++ky) {
-    const int oy = yb + ky;
-    if (oy < 0 || oy >= H) continue;
-    const float* row = d + (size_t)oy * W;
-    float r = 0.f;
-#pragma unroll
-    for (int kx = 0; kx < K; ++kx) {
-      const int ox = xb + kx;
-      if (ox >= 0 && ox < W) r = fmaf(wx[kx], __ldg(row + ox), r);
-    }
-    g = fmaf(wy[ky], r, g);
-  }
-  dsrc[t] = g;
+  resample_bwd_body<UP>(ddst, N, C, H, W, cout0, cin, Hs, Ws, dsrc);
 }
 
-// ---- depthwise 3x3 ------------------------------------------------------------------------------------------------------------------
-// y = scale * conv3x3(x, w[c]) (flip: the data gradient); a thread owns a 4-pixel column strip of `rows` consecutive rows.
 __global__ void __launch_bounds__(kT) dw3_kernel(const float* __restrict__ x, const float* __restrict__ w, float* __restrict__ y, int N, int C, int H,
                                                  int W, float scale, int flip, int quads, int rows) {
-  const int bands = (H + rows - 1) / rows;
-  const size_t t = (size_t)blockIdx.x * kT + threadIdx.x;
-  if (t >= (size_t)N * C * bands * quads) return;
-  const int q = (int)(t % quads), b = (int)((t / quads) % bands);
-  const size_t nc = t / ((size_t)quads * bands);
-  const int c = (int)(nc % C), x0 = 4 * q, r0 = b * rows, r1 = r0 + rows < H ? r0 + rows : H;
-  float k[9];
-#pragma unroll
-  for (int i = 0; i < 9; ++i) k[i] = __ldg(w + c * 9 + (flip ? 8 - i : i)) * scale;
-  const float* p = x + nc * H * W;
-  float* o = y + nc * H * W;
-  const bool vec = (W & 3) == 0;
-  float win[3][6];
-  auto load_row = [&](int r, float* d) {
-    if (r < 0 || r >= H) { d[0] = d[1] = d[2] = d[3] = d[4] = d[5] = 0.f; return; }
-    const float* s = p + (size_t)r * W + x0;
-    if (vec) {
-      const float4 m = __ldg(reinterpret_cast<const float4*>(s));
-      d[1] = m.x; d[2] = m.y; d[3] = m.z; d[4] = m.w;
-    } else {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) d[1 + j] = x0 + j < W ? __ldg(s + j) : 0.f;
-    }
-    d[0] = x0 > 0 ? __ldg(s - 1) : 0.f;
-    d[5] = x0 + 4 < W ? __ldg(s + 4) : 0.f;
-  };
-  load_row(r0 - 1, win[0]);
-  load_row(r0, win[1]);
-  for (int r = r0; r < r1; ++r) {
-    load_row(r + 1, win[2]);
-    float a[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float s = 0.f;
-#pragma unroll
-      for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-        for (int kx = 0; kx < 3; ++kx) s = fmaf(win[ky][j + kx], k[ky * 3 + kx], s);
-      a[j] = s;
-    }
-    float* d = o + (size_t)r * W + x0;
-    if (vec) *reinterpret_cast<float4*>(d) = make_float4(a[0], a[1], a[2], a[3]);
-    else {
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        if (x0 + j < W) d[j] = a[j];
-    }
-#pragma unroll
-    for (int j = 0; j < 6; ++j) { win[0][j] = win[1][j]; win[1][j] = win[2][j]; }
-  }
+  dw3_body(x, w, y, N, C, H, W, scale, flip, quads, rows);
 }
 
-// partial[block][c][9]: the block's share of sum_{n,y,x} dy[y][x] * x[y+ky-1][x+kx-1]; grid = (blocks per channel, C); a block walks
-// (image, band) units of its channel, a thread a 4-pixel strip of the band.
 __global__ void __launch_bounds__(kT) dw3_wgrad_kernel(const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ part, int N, int C,
                                                        int H, int W, int quads, int rows) {
-  const int c = blockIdx.y, bands = (H + rows - 1) / rows;
-  const size_t tasks = (size_t)N * bands * quads;
-  const bool vec = (W & 3) == 0;
-  float acc[9];
-#pragma unroll
-  for (int i = 0; i < 9; ++i) acc[i] = 0.f;
-  for (size_t t = (size_t)blockIdx.x * kT + threadIdx.x; t < tasks; t += (size_t)gridDim.x * kT) {
-    const int q = (int)(t % quads), b = (int)((t / quads) % bands), n = (int)(t / ((size_t)quads * bands));
-    const int x0 = 4 * q, r0 = b * rows, r1 = r0 + rows < H ? r0 + rows : H;
-    const float* p = x + ((size_t)n * C + c) * H * W;
-    const float* g = dy + ((size_t)n * C + c) * H * W;
-    float win[3][6];
-    auto load_row = [&](int r, float* d) {
-      if (r < 0 || r >= H) { d[0] = d[1] = d[2] = d[3] = d[4] = d[5] = 0.f; return; }
-      const float* s = p + (size_t)r * W + x0;
-      if (vec) {
-        const float4 m = __ldg(reinterpret_cast<const float4*>(s));
-        d[1] = m.x; d[2] = m.y; d[3] = m.z; d[4] = m.w;
-      } else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) d[1 + j] = x0 + j < W ? __ldg(s + j) : 0.f;
-      }
-      d[0] = x0 > 0 ? __ldg(s - 1) : 0.f;
-      d[5] = x0 + 4 < W ? __ldg(s + 4) : 0.f;
-    };
-    load_row(r0 - 1, win[0]);
-    load_row(r0, win[1]);
-    for (int r = r0; r < r1; ++r) {
-      load_row(r + 1, win[2]);
-      float d[4];
-      const float* gs = g + (size_t)r * W + x0;
-      if (vec) {
-        const float4 m = __ldg(reinterpret_cast<const float4*>(gs));
-        d[0] = m.x; d[1] = m.y; d[2] = m.z; d[3] = m.w;
-      } else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) d[j] = x0 + j < W ? __ldg(gs + j) : 0.f;
-      }
-#pragma unroll
-      for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-        for (int kx = 0; kx < 3; ++kx)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) acc[ky * 3 + kx] = fmaf(d[j], win[ky][j + kx], acc[ky * 3 + kx]);
-#pragma unroll
-      for (int j = 0; j < 6; ++j) { win[0][j] = win[1][j]; win[1][j] = win[2][j]; }
-    }
-  }
-  // block reduction in a fixed order: warp shuffles, then the 8 warp results
-  __shared__ float sh[kT / 32][9];
-#pragma unroll
-  for (int i = 0; i < 9; ++i) {
-    float v = acc[i];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5][i] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < 9) {
-    float s = 0.f;
-#pragma unroll
-    for (int wv = 0; wv < kT / 32; ++wv) s += sh[wv][threadIdx.x];
-    part[((size_t)blockIdx.x * C + c) * 9 + threadIdx.x] = s;
-  }
+  dw3_wgrad_body(x, dy, part, N, C, H, W, quads, rows);
 }
 
-// backward of the depthwise 3x3 in ONE pass over dy: dx = scale * conv3x3(dy, flipped w) and the block partials of
-// dw[c][tap] = sum dy[y][x] * x[y+ky-1][x+kx-1]; grid = (blocks per channel, C) as dw3_wgrad_kernel.
 __global__ void __launch_bounds__(kT) dw3_bwd_kernel(const float* __restrict__ x, const float* __restrict__ dy, const float* __restrict__ w,
                                                      float* __restrict__ dx, float* __restrict__ part, int N, int C, int H, int W, float scale,
                                                      int quads, int rows) {
-  const int c = blockIdx.y, bands = (H + rows - 1) / rows;
-  const size_t tasks = (size_t)N * bands * quads;
-  const bool vec = (W & 3) == 0;
-  float k[9], acc[9];
-#pragma unroll
-  for (int i = 0; i < 9; ++i) { k[i] = __ldg(w + c * 9 + 8 - i) * scale; acc[i] = 0.f; }
-  for (size_t t = (size_t)blockIdx.x * kT + threadIdx.x; t < tasks; t += (size_t)gridDim.x * kT) {
-    const int q = (int)(t % quads), b = (int)((t / quads) % bands), n = (int)(t / ((size_t)quads * bands));
-    const int x0 = 4 * q, r0 = b * rows, r1 = r0 + rows < H ? r0 + rows : H;
-    const size_t plane = ((size_t)n * C + c) * H * W;
-    const float* p = x + plane;
-    const float* g = dy + plane;
-    float* o = dx + plane;
-    float wx[3][6], wg[3][6];                                     // 3-row windows of x and dy, columns x0 - 1 ... x0 + 4
-    auto load_row = [&](const float* base, int r, float* d) {
-      if (r < 0 || r >= H) { d[0] = d[1] = d[2] = d[3] = d[4] = d[5] = 0.f; return; }
-      const float* s = base + (size_t)r * W + x0;
-      if (vec) {
-        const float4 m = __ldg(reinterpret_cast<const float4*>(s));
-        d[1] = m.x; d[2] = m.y; d[3] = m.z; d[4] = m.w;
-      } else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) d[1 + j] = x0 + j < W ? __ldg(s + j) : 0.f;
-      }
-      d[0] = x0 > 0 ? __ldg(s - 1) : 0.f;
-      d[5] = x0 + 4 < W ? __ldg(s + 4) : 0.f;
-    };
-    load_row(p, r0 - 1, wx[0]); load_row(p, r0, wx[1]);
-    load_row(g, r0 - 1, wg[0]); load_row(g, r0, wg[1]);
-    for (int r = r0; r < r1; ++r) {
-      load_row(p, r + 1, wx[2]);
-      load_row(g, r + 1, wg[2]);
-      float a[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float s = 0.f;
-#pragma unroll
-        for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-          for (int kx = 0; kx < 3; ++kx) s = fmaf(wg[ky][j + kx], k[ky * 3 + kx], s);
-        a[j] = s;
-      }
-      float* d = o + (size_t)r * W + x0;
-      if (vec) *reinterpret_cast<float4*>(d) = make_float4(a[0], a[1], a[2], a[3]);
-      else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (x0 + j < W) d[j] = a[j];
-      }
-#pragma unroll
-      for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-        for (int kx = 0; kx < 3; ++kx)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) acc[ky * 3 + kx] = fmaf(wg[1][1 + j], wx[ky][j + kx], acc[ky * 3 + kx]);
-#pragma unroll
-      for (int j = 0; j < 6; ++j) { wx[0][j] = wx[1][j]; wx[1][j] = wx[2][j]; wg[0][j] = wg[1][j]; wg[1][j] = wg[2][j]; }
-    }
-  }
-  __shared__ float sh[kT / 32][9];
-#pragma unroll
-  for (int i = 0; i < 9; ++i) {
-    float v = acc[i];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5][i] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < 9) {
-    float s = 0.f;
-#pragma unroll
-    for (int wv = 0; wv < kT / 32; ++wv) s += sh[wv][threadIdx.x];
-    part[((size_t)blockIdx.x * C + c) * 9 + threadIdx.x] = s;
-  }
+  dw3_bwd_body(x, dy, w, dx, part, N, C, H, W, scale, quads, rows);
 }
 
 }  // namespace tf

@@ -15,6 +15,7 @@
 #include "bce_sum.cuh"
 #include "generic_ops.cuh"
 #include "train_fast.cuh"
+#include "train_host.h"
 
 namespace {
 
@@ -27,156 +28,35 @@ int tfail(int code, const char* what, cudaError_t e);
 
 constexpr int kT = 256;
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
+using csnet::tf::block_sum3;
+using csnet::tf::warp_sum;
 
-// block-wide sum of up to 3 values; result valid in thread 0
-__device__ __forceinline__ void block_sum3(float& a, float& b, float& c) {
-  __shared__ float sh[3][kT / 32];
-  a = warp_sum(a); b = warp_sum(b); c = warp_sum(c);
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l == 0) { sh[0][w] = a; sh[1][w] = b; sh[2][w] = c; }
-  __syncthreads();
-  if (w == 0) {
-    a = l < kT / 32 ? sh[0][l] : 0.f; b = l < kT / 32 ? sh[1][l] : 0.f; c = l < kT / 32 ? sh[2][l] : 0.f;
-    a = warp_sum(a); b = warp_sum(b); c = warp_sum(c);
-  }
-  __syncthreads();
-}
-
-// ---- BatchNorm (train) + PReLU ---------------------------------------------------------------------------
-// Per-channel reductions over (N, H*W) run on a (C, parts) grid — a channel-per-block grid would leave most of the 132 SMs
-// idle for 8..79-channel layers.  A block reduces one segment of one image plane, publishes its partial to a workspace,
-// and the last block to arrive for a channel (ticket counter) merges the partials IN PART ORDER, so the result does not
-// depend on scheduling.  Segments: S per plane, parts = N * S.
-__device__ __forceinline__ bool last_block_of(unsigned* counter, unsigned parts) {
-  __shared__ bool is_last;
-  if (threadIdx.x == 0) {
-    __threadfence();
-    is_last = atomicAdd(counter, 1u) == parts - 1;
-  }
-  __syncthreads();
-  return is_last;
-}
-
-// stats: per channel mean and biased variance in ONE pass over z: sums of (z - K) and (z - K)^2 with the shift K = the mean of 32 fixed
-// samples spread over the channel's images and planes (every block of the channel computes the same K), so (mean - K)^2 ~ var / 32
-// and the subtraction S2 - S1^2 / M loses no more than a few ulps.  (A single sample is not enough: the corner pixel of a zero-padded
-// conv sits many sigma from the mean and cost 6e-3 on one weight gradient.)  Block partials in fp32 over <= a few hundred elements per
-// thread, merged in part order in double by the last block.
+// ---- BatchNorm (train) + PReLU: the fp32 instances of train_body.cuh's bodies ------------------------------------------------
 __global__ void __launch_bounds__(kT) bn_stats_kernel(const float* __restrict__ z, int N, int C, int HW, int S, float* mean,
                                                       float* var, float* ws, unsigned* cnt) {
-  const int c = blockIdx.x, part = blockIdx.y, parts = gridDim.y, n = part / S, sg = part - n * S;
-  const int seg = (HW + S - 1) / S, i0 = sg * seg, i1 = (i0 + seg) < HW ? (i0 + seg) : HW;
-  const float* p = z + ((size_t)n * C + c) * HW;
-  __shared__ float Ks;
-  if (threadIdx.x < 32) {
-    const int l = threadIdx.x, img = l % N, off = (int)(((long long)l * HW) / 32 + 17) % HW;
-    const float v = warp_sum(__ldg(z + ((size_t)img * C + c) * HW + off)) * (1.f / 32.f);
-    if (l == 0) Ks = v;
-  }
-  __syncthreads();
-  const float K = Ks;
-  float s = 0.f, q = 0.f, d1 = 0.f;
-  if (((HW | i0) & 3) == 0 && ((i1 - i0) & 3) == 0) {
-    const float4* p4 = reinterpret_cast<const float4*>(p + i0);
-    for (int i = threadIdx.x; i < (i1 - i0) / 4; i += kT) {
-      const float4 v = __ldg(p4 + i);
-      const float a = v.x - K, b = v.y - K, cc = v.z - K, d = v.w - K;
-      s += (a + b) + (cc + d);
-      q += (a * a + b * b) + (cc * cc + d * d);
-    }
-  } else {
-    for (int i = i0 + threadIdx.x; i < i1; i += kT) { const float d = p[i] - K; s += d; q += d * d; }
-  }
-  block_sum3(s, q, d1);
-  float* w = ws + ((size_t)c * parts + part) * 3;
-  if (threadIdx.x == 0) { w[0] = s; w[1] = q; w[2] = (float)(i1 > i0 ? i1 - i0 : 0); }
-  if (!last_block_of(cnt + c, parts)) return;
-  if (threadIdx.x == 0) {
-    __threadfence();
-    const volatile float* v = ws + (size_t)c * parts * 3;
-    double S1 = 0.0, S2 = 0.0, M = 0.0;
-    for (int k = 0; k < parts; ++k) { S1 += (double)v[3 * k]; S2 += (double)v[3 * k + 1]; M += (double)v[3 * k + 2]; }
-    const double m1 = S1 / M, vv = (S2 - S1 * m1) / M;
-    mean[c] = (float)((double)K + m1); var[c] = (float)(vv > 0.0 ? vv : 0.0);
-    cnt[c] = 0u;                                            // ready for the next call on this stream
-  }
+  csnet::tf::bn_stats_body(z, N, C, HW, S, mean, var, ws, cnt);
 }
 
-// y = prelu(gamma * (z - mean) * rsqrt(var + eps) + beta);  gap[n*C+c] = mean over HW of y (optional)
 __global__ void __launch_bounds__(kT) bn_prelu_fwd_kernel(const float* __restrict__ z, float* __restrict__ y, int C, int HW,
                                                           const float* mean, const float* var, const float* gamma,
                                                           const float* beta, const float* slope, float eps, float* gap) {
-  const int c = blockIdx.x, n = blockIdx.y;
-  const float r = rsqrtf(var[c] + eps), g = gamma[c] * r, b = beta[c] - mean[c] * g, a = slope[c];
-  const float* p = z + ((size_t)n * C + c) * HW;
-  float* o = y + ((size_t)n * C + c) * HW;
-  float s = 0.f, d0 = 0.f, d1 = 0.f;
-  for (int i = threadIdx.x; i < HW; i += kT) {
-    const float u = p[i] * g + b;
-    const float v = u > 0.f ? u : a * u;
-    o[i] = v;
-    s += v;
-  }
-  if (gap) {
-    block_sum3(s, d0, d1);
-    if (threadIdx.x == 0) gap[(size_t)n * C + c] = s / (float)HW;
-  }
+  csnet::tf::bn_prelu_fwd_body(z, y, C, HW, mean, var, gamma, beta, slope, eps, gap);
 }
 
-// backward reductions per channel: S1 = sum du, S2 = sum du * xhat, S3 = sum dy * u * [u <= 0]   (du = dy * prelu'(u));
-// same (C, parts) grid and ordered merge as bn_stats_kernel
 __global__ void __launch_bounds__(kT) bn_prelu_bwd_reduce_kernel(const float* __restrict__ z, const float* __restrict__ dy, int N,
                                                                  int C, int HW, int S, const float* mean, const float* var,
                                                                  const float* gamma, const float* beta, const float* slope,
                                                                  float eps, float* dgamma, float* dbeta, float* dslope, float* ws,
                                                                  unsigned* cnt) {
-  const int c = blockIdx.x, part = blockIdx.y, parts = gridDim.y, n = part / S, sg = part - n * S;
-  const int seg = (HW + S - 1) / S, i0 = sg * seg, i1 = (i0 + seg) < HW ? (i0 + seg) : HW;
-  const float mu = mean[c], r = rsqrtf(var[c] + eps), g = gamma[c], b = beta[c], a = slope[c];
-  float s1 = 0.f, s2 = 0.f, s3 = 0.f;
-  const float* p = z + ((size_t)n * C + c) * HW;
-  const float* q = dy + ((size_t)n * C + c) * HW;
-  for (int i = i0 + threadIdx.x; i < i1; i += kT) {
-    const float xh = (p[i] - mu) * r, u = g * xh + b, d = q[i];
-    const float du = u > 0.f ? d : a * d;
-    s1 += du; s2 += du * xh;
-    if (!(u > 0.f)) s3 += d * u;
-  }
-  block_sum3(s1, s2, s3);
-  float* w = ws + ((size_t)c * parts + part) * 3;
-  if (threadIdx.x == 0) { w[0] = s1; w[1] = s2; w[2] = s3; }
-  if (!last_block_of(cnt + c, parts)) return;
-  if (threadIdx.x == 0) {
-    __threadfence();
-    const volatile float* v = ws + (size_t)c * parts * 3;
-    float t1 = 0.f, t2 = 0.f, t3 = 0.f;
-    for (int k = 0; k < parts; ++k) { t1 += v[3 * k]; t2 += v[3 * k + 1]; t3 += v[3 * k + 2]; }
-    dbeta[c] = t1; dgamma[c] = t2; dslope[c] = t3;
-    cnt[c] = 0u;
-  }
+  csnet::tf::bn_prelu_bwd_reduce_body(z, dy, N, C, HW, S, mean, var, gamma, beta, slope, eps, dgamma, dbeta, dslope, ws, cnt);
 }
 
-// dz = gamma * r * (du - S1/M - xhat * S2/M)
 __global__ void __launch_bounds__(kT) bn_prelu_bwd_apply_kernel(const float* __restrict__ z, const float* __restrict__ dy,
                                                                 float* __restrict__ dz, int N, int C, int HW, const float* mean,
                                                                 const float* var, const float* gamma, const float* beta,
                                                                 const float* slope, float eps, const float* dgamma,
                                                                 const float* dbeta, int frozen) {
-  const int c = blockIdx.x, n = blockIdx.y;
-  const float mu = mean[c], r = rsqrtf(var[c] + eps), g = gamma[c], b = beta[c], a = slope[c];
-  // frozen statistics (eval-mode BN inside a training graph): mean / var are constants, no batch terms
-  const float invM = frozen ? 0.f : 1.f / ((float)N * (float)HW), m1 = dbeta[c] * invM, m2 = dgamma[c] * invM;
-  const size_t off = ((size_t)n * C + c) * HW;
-  for (int i = threadIdx.x; i < HW; i += kT) {
-    const float xh = (z[off + i] - mu) * r, u = g * xh + b, d = dy[off + i];
-    const float du = u > 0.f ? d : a * d;
-    dz[off + i] = g * r * (du - m1 - xh * m2);
-  }
+  csnet::tf::bn_prelu_bwd_apply_body(z, dy, dz, N, C, HW, mean, var, gamma, beta, slope, eps, dgamma, dbeta, frozen);
 }
 
 // ---- MIX forward (raw: no bias / slope) -----------------------------------------------------------------------
@@ -367,14 +247,6 @@ int tfail(int code, const char* what, cudaError_t e) {
   return code;
 }
 
-csnet::MixPath to_path(const csnet_train_path& q) {
-  csnet::MixPath m{};
-  m.src = q.src; m.w = q.w; m.dtype = CSNET_F32; m.C = q.C; m.H = q.H; m.W = q.W; m.c0 = q.c0; m.cin = q.cin;
-  m.pre_avg = q.pre_avg; m.pool = q.pool; m.ksize = q.ksize; m.dil = q.dil; m.stride = q.stride; m.pad = q.pad; m.up = q.up;
-  m.cout0 = q.cout0; m.cout = q.cout;
-  return m;
-}
-
 // ---- SalMetric counting (sal_metric.cpp:86-120): per-image 256-bin histograms of the quantised saliency ----------------
 __global__ void __launch_bounds__(kT) salmetric_hist_kernel(const float* __restrict__ prob, const uint8_t* __restrict__ gt, int64_t HW,
                                                             uint32_t* hist_all, uint32_t* hist_pos, unsigned long long* abs_sum) {
@@ -403,24 +275,26 @@ __global__ void __launch_bounds__(kT) salmetric_hist_kernel(const float* __restr
 }  // namespace
 
 namespace csnet {
-// The other training sources (train_csf.cu, plan.cu's resize pair) report through csnet_train_last_error too.
+// The other training sources (train_csf.cu, train_bf16.cu, plan.cu's resize pair) report through csnet_train_last_error too.
 void train_set_error(const char* msg) { t_err = msg; }
-}  // namespace csnet
 
-extern "C" {
+namespace tr {
 
-const char* csnet_train_last_error(void) { return t_err.c_str(); }
+MixPath to_path(const csnet_train_path& q) {
+  csnet::MixPath m{};
+  m.src = q.src; m.w = q.w; m.dtype = CSNET_F32; m.C = q.C; m.H = q.H; m.W = q.W; m.c0 = q.c0; m.cin = q.cin;
+  m.pre_avg = q.pre_avg; m.pool = q.pool; m.ksize = q.ksize; m.dil = q.dil; m.stride = q.stride; m.pad = q.pad; m.up = q.up;
+  m.cout0 = q.cout0; m.cout = q.cout;
+  return m;
+}
 
 // Workspace of the channel reductions: partials [C][parts][3] + one ticket counter per channel.  One set PER DEVICE (indexed by
 // the current device, i.e. the device of the tensors the caller's torch stream belongs to), grown on demand; the training entry
 // points of one device are meant to be issued on ONE stream (calls serialise there, so sharing within a device is safe).
-constexpr int kMaxDevices = 16;
 struct RedWs { float* ws = nullptr; unsigned* cnt = nullptr; size_t ws_cap = 0, cnt_cap = 0; float* part = nullptr; size_t part_cap = 0; };
 static RedWs g_red[kMaxDevices];
-static thread_local float* g_red_ws = nullptr;          // the current call's workspace (set by reduce_workspace)
-static thread_local unsigned* g_red_cnt = nullptr;
 
-static int reduce_workspace(int C, int parts, cudaStream_t st) {
+int reduce_workspace(int C, int parts, cudaStream_t st, float** ws, unsigned** cnt) {
   int dev = 0;
   TR_CHECK(cudaGetDevice(&dev));
   if (dev < 0 || dev >= kMaxDevices) { t_err = "device index out of range"; return CSNET_E_INVALID; }
@@ -442,13 +316,13 @@ static int reduce_workspace(int C, int parts, cudaStream_t st) {
     TR_CHECK(cudaMemset(R.cnt, 0, cap * sizeof(unsigned)));
     R.cnt_cap = cap;
   }
-  g_red_ws = R.ws;
-  g_red_cnt = R.cnt;
+  *ws = R.ws;
+  *cnt = R.cnt;
   return CSNET_OK;
 }
 
 // Block partials of the weight-gradient kernels ([blocks][elements] floats), one buffer per device, grown on demand.
-static int partial_workspace(size_t floats, cudaStream_t st, float** out) {
+int partial_workspace(size_t floats, cudaStream_t st, float** out) {
   int dev = 0;
   TR_CHECK(cudaGetDevice(&dev));
   if (dev < 0 || dev >= kMaxDevices) { t_err = "device index out of range"; return CSNET_E_INVALID; }
@@ -466,18 +340,14 @@ static int partial_workspace(size_t floats, cudaStream_t st, float** out) {
 }
 
 // ---- fast (register-tiled) dispatch: train_fast.cuh ------------------------------------------------------------------------------
-namespace tf = csnet::tf;
-constexpr size_t kFastSmem = 92 * 1024;                   // operand tiles; + kFastWsm of weights: two blocks per SM
-constexpr size_t kFastWsm = 16 * 1024;
-constexpr int kFastSmemMax = (int)(kFastSmem + kFastWsm);
 
-static int current_device() {
+int current_device() {
   int dev = 0;
   cudaGetDevice(&dev);
   return dev < 0 || dev >= kMaxDevices ? 0 : dev;
 }
 
-static int num_sms() {
+int num_sms() {
   static int sms[kMaxDevices] = {0};
   int dev = 0;
   cudaGetDevice(&dev);
@@ -486,7 +356,7 @@ static int num_sms() {
   return sms[dev] > 0 ? sms[dev] : 132;
 }
 
-static bool conv_tile_geometry(tf::ConvArgs& A) {
+bool conv_tile_geometry(tf::ConvArgs& A) {
   A.quads = (A.W + 3) / 4;
   A.vec = (A.W % 4) == 0;
   if (A.quads > tf::kT) return false;
@@ -496,13 +366,13 @@ static bool conv_tile_geometry(tf::ConvArgs& A) {
   return true;
 }
 
-static bool conv_path_geometry(tf::ConvPath& P, const tf::ConvArgs& A) {
+bool conv_path_geometry(tf::ConvPath& P, const tf::ConvArgs& A, int esize) {
   const int kk = A.ksize * A.ksize;
   P.halo = P.dil * (A.ksize / 2);
   P.hp = (P.halo + 3) / 4 * 4;
   P.Wp = (A.W + 2 * P.hp + 3) / 4 * 4;
   P.rows = A.R + 2 * P.halo;
-  const size_t per_ci = (size_t)A.ipb * P.rows * P.Wp * sizeof(float), per_w = (size_t)kk * tf::kCoT * sizeof(float);
+  const size_t per_ci = (size_t)A.ipb * P.rows * P.Wp * esize, per_w = (size_t)kk * tf::kCoT * sizeof(float);
   size_t chunk = kFastSmem / per_ci;
   if (chunk > kFastWsm / per_w) chunk = kFastWsm / per_w;
   if (chunk < 1) return false;
@@ -510,7 +380,74 @@ static bool conv_path_geometry(tf::ConvPath& P, const tf::ConvArgs& A) {
   return true;
 }
 
-constexpr int kNotHandled = 1;                            // the shape does not fit the fast kernel: the caller runs the generic one
+bool dense_conv_path(const csnet::MixPath& P, int H, int W) {
+  return P.ksize >= 1 && (P.ksize & 1) && P.stride == 1 && P.pre_avg == 0 && P.pool == 1 && P.up == 1 && P.H == H && P.W == W &&
+         P.pad == P.dil * (P.ksize / 2) && P.dil >= 1;
+}
+
+// segments per image plane: enough parts to fill the GPU for narrow layers and small batches, at most 64 per plane
+int reduce_segments(int N, int C, int HW) {
+  int S = 1;
+  while ((long)N * C * S < 1184 && S < 64 && HW / (S * 2) >= 2048) S *= 2;
+  return S;
+}
+
+// Geometry of the register-tiled weight gradient of one dense path (3x3 at any dilation, or 1x1 at dilation 1); false: the
+// shape is not taken.  esize_in / esize_dd: bytes per element of the source and of the destination gradient.
+bool wgrad_plan(const MixPath& P, const void* ddst, int N, int C, int H, int W, int esize_in, int esize_dd, WgradPlan& out) {
+  if (!(dense_conv_path(P, H, W) && (P.ksize == 3 || (P.ksize == 1 && P.dil == 1)))) return false;
+  const int kk = P.ksize * P.ksize;
+  const int form = P.ksize == 1 ? 1 : (P.dil == 1 ? 3 : 0);    // template argument of conv_wgrad_kernel
+  tf::WgradArgs G{};
+  G.in = P.src; G.dd = ddst; G.N = N; G.Cs = P.C; G.c0 = P.c0; G.cin = P.cin; G.Cd = C; G.cout0 = P.cout0;
+  G.cout = P.cout; G.H = H; G.W = W; G.dil = P.dil;
+  G.cin4 = (P.cin + 3) / 4 * 4; G.cout4 = (P.cout + 3) / 4 * 4;
+  G.hp = form == 0 ? (P.dil + 3) / 4 * 4 : 4;
+  G.Wp = (W + 2 * G.hp + 3) / 4 * 4; G.quads = (W + 3) / 4; G.vec = (W % 4) == 0;
+  auto rows_in = [&](int r) { return form == 0 ? 3 * r : r + (form == 3 ? 2 : 0); };
+  auto pitch = [](int elems) { return elems + ((4 - elems % 32) + 32) % 32; };          // == 4 (mod 32); elems is a multiple of 4
+  auto stage_bytes = [&](int r) {
+    return (size_t)G.cin4 * pitch(rows_in(r) * G.Wp) * esize_in + (size_t)G.cout4 * pitch(r * G.Wp) * esize_dd;
+  };
+  int R = 0;                                               // the largest row band whose operands fit
+  for (int r = 1; r <= H && r <= 16; ++r)
+    if (stage_bytes(r) <= kFastSmemMax / 2) R = r;        // two stages in flight
+  if (R < 1) return false;
+  G.R = R;
+  G.cpi = pitch(rows_in(R) * G.Wp); G.cpd = pitch(R * G.Wp);
+  const int bands = (H + R - 1) / R;
+  G.units = N * bands;
+  G.mt = G.cin4 / 4 * (form == 1 ? 1 : 3); G.nt = G.cout4 / 4; G.tiles = G.mt * G.nt;
+  int groups = 1;
+  if (G.tiles <= tf::kT) {
+    if (G.tiles >= 32) G.tpad = (G.tiles + 31) / 32 * 32;
+    else { G.tpad = 1; while (G.tpad < G.tiles) G.tpad *= 2; }
+    G.splits = tf::kT / G.tpad;
+  } else {
+    G.tpad = tf::kT; G.splits = 1; groups = (G.tiles + tf::kT - 1) / tf::kT;
+  }
+  const size_t stage = stage_bytes(R),
+               red = (size_t)G.splits * G.tpad * (form == 1 ? 16 : 48) * sizeof(float);
+  int gx = 2 * num_sms() / groups;
+  gx = gx < 1 ? 1 : gx;
+  gx = gx > G.units ? G.units : gx;
+  out.A = G;
+  out.form = form; out.gx = gx; out.groups = groups; out.nel = P.cin * kk * P.cout;
+  out.smem = 2 * stage > red ? 2 * stage : red;
+  return true;
+}
+
+int reduce_partials(const float* part, int parts, int n, float scale, float* out, cudaStream_t st) {
+  tf::reduce_partials_kernel<<<(n + tf::kT - 1) / tf::kT, tf::kT, 0, st>>>(part, parts, n, scale, out);
+  TR_CHECK(cudaGetLastError());
+  return CSNET_OK;
+}
+
+}  // namespace tr
+}  // namespace csnet
+
+using namespace csnet::tr;
+
 // 1x1 mixes (and mixes of resample-add paths only): the direct kernel
 static int launch_conv1x1(const tf::ConvArgs& F, cudaStream_t st) {
   tf::C1Args A{};
@@ -587,17 +524,13 @@ static int launch_conv(tf::ConvArgs& A, cudaStream_t st) {
   return CSNET_OK;
 }
 
-static bool dense_conv_path(const csnet::MixPath& P, int H, int W) {
-  return P.ksize >= 1 && (P.ksize & 1) && P.stride == 1 && P.pre_avg == 0 && P.pool == 1 && P.up == 1 && P.H == H && P.W == W &&
-         P.pad == P.dil * (P.ksize / 2) && P.dil >= 1;
-}
+static thread_local float* g_red_ws = nullptr;          // the current call's workspace (set by reduce_workspace)
+static thread_local unsigned* g_red_cnt = nullptr;
+static int reduce_workspace(int C, int parts, cudaStream_t st) { return csnet::tr::reduce_workspace(C, parts, st, &g_red_ws, &g_red_cnt); }
 
-// segments per image plane: enough parts to fill the GPU for narrow layers and small batches, at most 64 per plane
-static int reduce_segments(int N, int C, int HW) {
-  int S = 1;
-  while ((long)N * C * S < 1184 && S < 64 && HW / (S * 2) >= 2048) S *= 2;
-  return S;
-}
+extern "C" {
+
+const char* csnet_train_last_error(void) { return t_err.c_str(); }
 
 int csnet_train_bn_stats(const float* z, int32_t N, int32_t C, int32_t HW, float* mean, float* var, void* stream) {
   const int S = reduce_segments(N, C, HW);
@@ -693,7 +626,7 @@ int csnet_train_mix_fwd(float* dst, int32_t N, int32_t C, int32_t H, int32_t W, 
   }
   if (ok) {
     F.ksize = ks ? ks : 1;
-    for (int i = 0; i < F.n_conv && ok; ++i) ok = conv_path_geometry(F.p[i], F);
+    for (int i = 0; i < F.n_conv && ok; ++i) ok = conv_path_geometry(F.p[i], F, sizeof(float));
   }
   if (ok) {
     const int rc = launch_conv(F, (cudaStream_t)stream);
@@ -720,7 +653,7 @@ int csnet_train_mix_dgrad(const float* ddst, int32_t N, int32_t C, int32_t H, in
     F.dst = dsrc; F.N = N; F.C = P.cin; F.H = H; F.W = W; F.ksize = P.ksize; F.transposed = 1; F.n_conv = 1;
     tf::ConvPath& Q = F.p[0];
     Q.src = ddst; Q.w = P.w; Q.Cs = C; Q.c0 = P.cout0; Q.cin = P.cout; Q.cout0 = 0; Q.cout = P.cin; Q.dil = P.dil;
-    if (conv_tile_geometry(F) && conv_path_geometry(Q, F)) {
+    if (conv_tile_geometry(F) && conv_path_geometry(Q, F, sizeof(float))) {
       const int rc = launch_conv(F, (cudaStream_t)stream);
       if (rc != kNotHandled) return rc;
     }
@@ -735,60 +668,25 @@ int csnet_train_mix_wgrad(const float* ddst, int32_t N, int32_t C, int32_t H, in
   if (P.ksize == 0) { t_err = "csnet_train_mix_wgrad: resample paths have no weights"; return CSNET_E_INVALID; }
   if (P.pre_avg > 2 || P.up > 1) { t_err = "csnet_train_mix_wgrad: down-sample factors > 2 / input-side up-sampling are inference-only"; return CSNET_E_UNSUPPORTED; }
   const int kk = P.ksize * P.ksize;
-  if (dense_conv_path(P, H, W) && (P.ksize == 3 || (P.ksize == 1 && P.dil == 1))) {
-    const int form = P.ksize == 1 ? 1 : (P.dil == 1 ? 3 : 0);    // template argument of conv_wgrad_kernel
-    tf::WgradArgs G{};
-    G.in = reinterpret_cast<const float*>(P.src); G.dd = ddst; G.N = N; G.Cs = P.C; G.c0 = P.c0; G.cin = P.cin; G.Cd = C; G.cout0 = P.cout0;
-    G.cout = P.cout; G.H = H; G.W = W; G.dil = P.dil;
-    G.cin4 = (P.cin + 3) / 4 * 4; G.cout4 = (P.cout + 3) / 4 * 4;
-    G.hp = form == 0 ? (P.dil + 3) / 4 * 4 : 4;
-    G.Wp = (W + 2 * G.hp + 3) / 4 * 4; G.quads = (W + 3) / 4; G.vec = (W % 4) == 0;
-    auto rows_in = [&](int r) { return form == 0 ? 3 * r : r + (form == 3 ? 2 : 0); };
-    auto pitch = [](int floats) { return floats + ((4 - floats % 32) + 32) % 32; };          // == 4 (mod 32); floats is a multiple of 4
-    auto stage_bytes = [&](int r) { return ((size_t)G.cin4 * pitch(rows_in(r) * G.Wp) + (size_t)G.cout4 * pitch(r * G.Wp)) * sizeof(float); };
-    int R = 0;                                               // the largest row band whose operands fit
-    for (int r = 1; r <= H && r <= 16; ++r)
-      if (stage_bytes(r) <= kFastSmemMax / 2) R = r;        // two stages in flight
-    if (R >= 1) {
-      G.R = R;
-      G.cpi = pitch(rows_in(R) * G.Wp); G.cpd = pitch(R * G.Wp);
-      const int bands = (H + R - 1) / R;
-      G.units = N * bands;
-      G.mt = G.cin4 / 4 * (form == 1 ? 1 : 3); G.nt = G.cout4 / 4; G.tiles = G.mt * G.nt;
-      int groups = 1;
-      if (G.tiles <= tf::kT) {
-        if (G.tiles >= 32) G.tpad = (G.tiles + 31) / 32 * 32;
-        else { G.tpad = 1; while (G.tpad < G.tiles) G.tpad *= 2; }
-        G.splits = tf::kT / G.tpad;
-      } else {
-        G.tpad = tf::kT; G.splits = 1; groups = (G.tiles + tf::kT - 1) / tf::kT;
-      }
-      const size_t stage = stage_bytes(R),
-                   red = (size_t)G.splits * G.tpad * (form == 1 ? 16 : 48) * sizeof(float);
-      const size_t smem = 2 * stage > red ? 2 * stage : red;
-      int gx = 2 * num_sms() / groups;
-      gx = gx < 1 ? 1 : gx;
-      gx = gx > G.units ? G.units : gx;
-      const int nel = P.cin * kk * P.cout;
-      float* part = nullptr;
-      if (int rc = partial_workspace((size_t)gx * nel, (cudaStream_t)stream, &part)) return rc;
-      G.part = part;
-      static bool attr_dev[kMaxDevices] = {false};
-      bool& attr = attr_dev[current_device()];
-      if (!attr) {
-        cudaFuncSetAttribute(tf::conv_wgrad_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFastSmemMax);
-        cudaFuncSetAttribute(tf::conv_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFastSmemMax);
-        cudaFuncSetAttribute(tf::conv_wgrad_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFastSmemMax);
-        attr = true;
-      }
-      if (form == 1) tf::conv_wgrad_kernel<1><<<dim3(gx, groups), tf::kT, smem, (cudaStream_t)stream>>>(G);
-      else if (form == 3) tf::conv_wgrad_kernel<3><<<dim3(gx, groups), tf::kT, smem, (cudaStream_t)stream>>>(G);
-      else tf::conv_wgrad_kernel<0><<<dim3(gx, groups), tf::kT, smem, (cudaStream_t)stream>>>(G);
-      TR_CHECK(cudaGetLastError());
-      tf::reduce_partials_kernel<<<(nel + tf::kT - 1) / tf::kT, tf::kT, 0, (cudaStream_t)stream>>>(part, gx, nel, 1.f, dw);
-      TR_CHECK(cudaGetLastError());
-      return CSNET_OK;
+  WgradPlan G;
+  if (wgrad_plan(P, ddst, N, C, H, W, sizeof(float), sizeof(float), G)) {
+    float* part = nullptr;
+    if (int rc = partial_workspace((size_t)G.gx * G.nel, (cudaStream_t)stream, &part)) return rc;
+    G.A.part = part;
+    static bool attr_dev[kMaxDevices] = {false};
+    bool& attr = attr_dev[current_device()];
+    if (!attr) {
+      cudaFuncSetAttribute(tf::conv_wgrad_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFastSmemMax);
+      cudaFuncSetAttribute(tf::conv_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFastSmemMax);
+      cudaFuncSetAttribute(tf::conv_wgrad_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFastSmemMax);
+      attr = true;
     }
+    const dim3 grid(G.gx, G.groups);
+    if (G.form == 1) tf::conv_wgrad_kernel<1><<<grid, tf::kT, G.smem, (cudaStream_t)stream>>>(G.A);
+    else if (G.form == 3) tf::conv_wgrad_kernel<3><<<grid, tf::kT, G.smem, (cudaStream_t)stream>>>(G.A);
+    else tf::conv_wgrad_kernel<0><<<grid, tf::kT, G.smem, (cudaStream_t)stream>>>(G.A);
+    TR_CHECK(cudaGetLastError());
+    return reduce_partials(part, G.gx, G.nel, 1.f, dw, (cudaStream_t)stream);
   }
   TR_CHECK(cudaMemsetAsync(dw, 0, (size_t)P.cin * kk * P.cout * sizeof(float), (cudaStream_t)stream));
   const int split = N < 32 ? N : 32;

@@ -148,11 +148,20 @@ def ms_block_forward(m, x):
 
 
 def csnet_forward(model, x):
-    """CSNet.forward (csnet.py:365-387) on the module-granular kernels."""
+    """CSNet.forward (csnet.py:365-387) on the module-granular kernels.
+
+    Activation storage (`model.train_storage`, set by Trainer(storage=...)): "fp32" (default) or "bf16".  In bf16 every
+    activation a module passes on or saves for backward, and its gradient, is bf16: conv outputs, BN + PReLU outputs,
+    depthwise outputs and pooled copies of bf16 sources.  The network input, the stem's max-pooled input, the 1-channel maps
+    after cls_layer, the logits and the loss stay fp32, and so do parameters, their gradients and the BatchNorm statistics."""
     if not x.is_cuda:
         raise T.runtime.EngineError("CSNet (CUDA engine) needs CUDA tensors; there is no CPU path")
     if x.shape[2] % 16 or x.shape[3] % 16:
         raise ValueError(f"input size {tuple(x.shape[2:])} must be a multiple of 16")
+    storage = getattr(model, "train_storage", "fp32")
+    if storage not in T.STORAGES:
+        raise ValueError(f"train_storage must be one of {sorted(T.STORAGES)}, got {storage!r}")
+    dt = T.STORAGES[storage]
     feats, cur = {}, [x.float()]
     # recompute mode (Trainer(recompute=True) / model.recompute = True): an ILBlock keeps only its inputs; its six modules' saved tensors
     # (conv outputs, BN inputs, pooled copies) are rebuilt block by block in the backward pass — ~3.4x less activation memory for one
@@ -161,16 +170,18 @@ def csnet_forward(model, x):
     if ckpt:
         import contextlib
         from torch.utils.checkpoint import checkpoint
-        ctx = lambda: (contextlib.nullcontext(), T.recomputing())
-    for s in range(5):
-        for blk in getattr(model, f"stage{s}"):
-            cur = checkpoint(blk, cur, use_reentrant=False, context_fn=ctx) if ckpt else blk(cur)
-        feats[s] = cur
-    fuse = model.oct_fuse([feats[2][0], feats[3][0], feats[4][0]])
+        ctx = lambda: (contextlib.nullcontext(), T.recomputing(dt))       # the re-run stores what the first run stored
+    with T.storage(dt):
+        for s in range(5):
+            for blk in getattr(model, f"stage{s}"):
+                cur = checkpoint(blk, cur, use_reentrant=False, context_fn=ctx) if ckpt else blk(cur)
+            feats[s] = cur
+        fuse = model.oct_fuse([feats[2][0], feats[3][0], feats[4][0]])
     cls = model.cls_layer
     w = T.pack_conv_weight(cls.weight)
     f0 = fuse[0]
-    low = T.MixFn.apply((cls.out_channels, f0.shape[2], f0.shape[3], [T.PathSpec(0, 1, f0.shape[1], cls.out_channels, ksize=1)]), f0, w)
-    low = low + cls.bias.view(1, -1, 1, 1)
-    up = x.shape[2] // f0.shape[2]
-    return T.MixFn.apply((cls.out_channels, x.shape[2], x.shape[3], [T.PathSpec(0, None, cls.out_channels, cls.out_channels, ksize=0, up=up)]), low)
+    with T.storage(torch.float32):                      # cls_layer writes fp32: the 1-channel maps and the logits stay fp32
+        low = T.MixFn.apply((cls.out_channels, f0.shape[2], f0.shape[3], [T.PathSpec(0, 1, f0.shape[1], cls.out_channels, ksize=1)]), f0, w)
+        low = low + cls.bias.view(1, -1, 1, 1)
+        up = x.shape[2] // f0.shape[2]
+        return T.MixFn.apply((cls.out_channels, x.shape[2], x.shape[3], [T.PathSpec(0, None, cls.out_channels, cls.out_channels, ksize=0, up=up)]), low)

@@ -1,7 +1,9 @@
 """Training primitives: ctypes bindings of the `csnet_train_*` C ABI wrapped as torch.autograd.Function s.
 
 torch is plumbing here (tensor storage, the autograd tape, tiny parameter reshapes); every kernel that touches an
-activation is ours.  fp32 activations (the parity configuration); see DESIGN.md for the bf16 plan.
+activation is ours.  Activations are stored in fp32 (the parity configuration, the default) or in bf16: each Function follows
+the dtype of the activations it receives and picks the fp32 or the `_bf16` entry points from it; weights, weight gradients and
+BatchNorm statistics are fp32 either way.
 """
 from __future__ import annotations
 
@@ -12,7 +14,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
-from . import runtime
+from . import ir, runtime
 
 BN_EPS = 1e-5
 
@@ -46,8 +48,40 @@ def lib():
         l.csnet_train_pool_bwd.argtypes = [f32p, vp, i32, i32, i32, i32, i32, i32, f32p, vp]
         l.csnet_train_bce.argtypes = [f32p, f32p, f32p, f32p, i64, f, vp]
         l.csnet_train_adam.argtypes = [vp, i32, f, f, f, f, i32, f, vp]
+        l.csnet_train_bn_stats_bf16.argtypes = [vp, i32, i32, i32, f32p, f32p, vp]
+        l.csnet_train_bn_prelu_fwd_bf16.argtypes = [vp, vp, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, f, f32p, vp]
+        l.csnet_train_bn_prelu_bwd_bf16.argtypes = [vp, vp, vp, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, f, f32p, f32p, f32p, i32, vp]
+        l.csnet_train_dw_conv_bf16.argtypes = [vp, f32p, vp, i32, i32, i32, i32, f, i32, vp]
+        l.csnet_train_dw_wgrad_bf16.argtypes = [vp, vp, f32p, i32, i32, i32, i32, f, vp]
+        l.csnet_train_dw_bwd_bf16.argtypes = [vp, vp, f32p, vp, f32p, i32, i32, i32, i32, f, vp]
+        l.csnet_train_mix_fwd_bf16.argtypes = [vp, i32, i32, i32, i32, i32, C.POINTER(TrainPath), i32, i32, vp]
+        l.csnet_train_mix_dgrad_bf16.argtypes = [vp, i32, i32, i32, i32, i32, C.POINTER(TrainPath), vp, i32, vp]
+        l.csnet_train_mix_wgrad_bf16.argtypes = [vp, i32, i32, i32, i32, i32, C.POINTER(TrainPath), f32p, i32, vp]
+        l.csnet_train_pool_fwd_bf16.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, vp, vp]
+        l.csnet_train_pool_bwd_bf16.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, vp, vp]
         _lib = l
     return _lib
+
+
+# Activation storage of the module-granular forward (modular.csnet_forward sets it for a training step): the dtype a MixFn writes
+# unless its spec names one.  DwFn and BnPreluFn follow the dtype of their input.
+STORAGE = torch.float32
+STORAGES = {"fp32": torch.float32, "bf16": torch.bfloat16}
+
+
+class storage:
+    """The activation storage dtype of the MixFns run inside the block."""
+
+    def __init__(self, dtype):
+        self.dtype = dtype
+
+    def __enter__(self):
+        global STORAGE
+        self._old, STORAGE = STORAGE, self.dtype
+
+    def __exit__(self, *exc):
+        global STORAGE
+        STORAGE = self._old
 
 
 # True while a checkpointed ILBlock is being re-run in the backward pass (modular.csnet_forward with recompute): the second run must
@@ -56,18 +90,27 @@ RECOMPUTING = False
 
 
 class recomputing:
+    """The re-run of a checkpointed block; `storage` (a dtype): the activation storage of that re-run."""
+
+    def __init__(self, storage=None):
+        self.storage = storage
+
     def __enter__(self):
-        global RECOMPUTING
+        global RECOMPUTING, STORAGE
         self._old, RECOMPUTING = RECOMPUTING, True
+        self._old_storage = STORAGE
+        if self.storage is not None:
+            STORAGE = self.storage
 
     def __exit__(self, *exc):
-        global RECOMPUTING
-        RECOMPUTING = self._old
+        global RECOMPUTING, STORAGE
+        RECOMPUTING, STORAGE = self._old, self._old_storage
 
 
 # kernels launched through this module since import (bench.py reports the count of a timed region): kernels per entry point
 LAUNCHES = 0
-_KERNELS = {"csnet_train_bn_prelu_bwd": 2, "csnet_train_mix_wgrad": 2, "csnet_train_dw_wgrad": 2, "csnet_train_dw_bwd": 2}
+_KERNELS = {"csnet_train_bn_prelu_bwd": 2, "csnet_train_mix_wgrad": 2, "csnet_train_dw_wgrad": 2, "csnet_train_dw_bwd": 2,
+            "csnet_train_bn_prelu_bwd_bf16": 2, "csnet_train_mix_wgrad_bf16": 2, "csnet_train_dw_wgrad_bf16": 2, "csnet_train_dw_bwd_bf16": 2}
 
 
 def _ck(rc, what):
@@ -85,6 +128,19 @@ def _f32(t: torch.Tensor) -> torch.Tensor:
     if not t.is_cuda:
         raise runtime.EngineError("training runs on the GPU only: got a CPU tensor")
     return t.contiguous().float()
+
+
+def _act(t: torch.Tensor) -> torch.Tensor:
+    """An activation as the kernels read it: bf16 stays bf16, anything else becomes fp32."""
+    if t.dtype == torch.bfloat16:
+        if not t.is_cuda:
+            raise runtime.EngineError("training runs on the GPU only: got a CPU tensor")
+        return t.contiguous()
+    return _f32(t)
+
+
+def _code(dtype) -> int:
+    return ir.BF16 if dtype == torch.bfloat16 else ir.F32           # CSNET_BF16 / CSNET_F32
 
 
 # ---- raw conv mix ------------------------------------------------------------------------------------------------
@@ -114,14 +170,24 @@ def _cpath(ps: PathSpec, tensors: Sequence[torch.Tensor]) -> TrainPath:
 class MixFn(torch.autograd.Function):
     """dst[N, C, H, W] = sum of paths (gOctaveConv.forward for one output branch, csnet.py:664-726).
 
+    spec = (C, H, W, paths[, dtype]): dst has `dtype`, else the storage in effect (STORAGE).  The sources of one mix share a
+    dtype (fp32 or bf16); a call with bf16 on either side runs on the `_bf16` entry points, gradients in the sources' dtype.
+
     The down-sampling of a path (2x2 average of a stride-2 conv, max-pool of a high -> low path) is materialised once by
     csnet_train_pool_fwd, with the arg-max; the convolution kernels then see dense stride-1 paths only, the backward routes the
     pooled gradient with csnet_train_pool_bwd, and the full-resolution source is not kept for this Function."""
 
     @staticmethod
     def forward(ctx, spec, *tensors):
-        out_c, out_h, out_w, paths = spec
-        tensors = [_f32(t) for t in tensors]
+        out_c, out_h, out_w, paths = spec[:4]
+        srcs = {p.src for p in paths}
+        tensors = [_act(t) if i in srcs else _f32(t) for i, t in enumerate(tensors)]
+        sdt = {tensors[i].dtype for i in srcs}
+        if len(sdt) != 1:
+            raise runtime.EngineError(f"MixFn: the sources of one mix must share a dtype, got {sorted(map(str, sdt))}")
+        sdt = sdt.pop()
+        odt = spec[4] if len(spec) > 4 else STORAGE        # destination dtype: the spec's, else the storage in effect
+        bf = torch.bfloat16 in (sdt, odt)
         n = tensors[paths[0].src].shape[0]
         dev = tensors[0].device
         st = torch.cuda.current_stream(dev).cuda_stream
@@ -131,18 +197,23 @@ class MixFn(torch.autograd.Function):
             if p.ksize > 0 and (p.pre_avg or p.pool > 1):
                 s = tensors[p.src]
                 f = (2 if p.pre_avg else 1) * p.pool
-                xp = torch.empty((n, p.cin, s.shape[2] // f, s.shape[3] // f), dtype=torch.float32, device=dev)
+                xp = torch.empty((n, p.cin, s.shape[2] // f, s.shape[3] // f), dtype=sdt, device=dev)     # a pooled copy has its source's dtype
                 idx = torch.empty(xp.shape, dtype=torch.uint8, device=dev) if p.pool > 1 else None
-                _ck(lib().csnet_train_pool_fwd(s.data_ptr(), n, s.shape[1], p.c0, p.cin, s.shape[2], s.shape[3], p.pre_avg, p.pool,
-                                               xp.data_ptr(), idx.data_ptr() if idx is not None else None, st), "csnet_train_pool_fwd")
+                fn = "csnet_train_pool_fwd_bf16" if sdt == torch.bfloat16 else "csnet_train_pool_fwd"
+                _ck(getattr(lib(), fn)(s.data_ptr(), n, s.shape[1], p.c0, p.cin, s.shape[2], s.shape[3], p.pre_avg, p.pool,
+                                       xp.data_ptr(), idx.data_ptr() if idx is not None else None, st), fn)
                 saved += [xp, idx]
                 pooled[k] = (len(saved) - 2, len(saved) - 1, tuple(s.shape))
                 dense.append(PathSpec(len(saved) - 2, p.w, p.cin, p.cout, cout0=p.cout0, ksize=p.ksize, dil=p.dil, stride=p.stride, pad=p.pad))
             else:
                 dense.append(p)
-        dst = torch.empty((n, out_c, out_h, out_w), dtype=torch.float32, device=dev)
+        dst = torch.empty((n, out_c, out_h, out_w), dtype=odt, device=dev)
         arr = (TrainPath * len(dense))(*[_cpath(p, saved) for p in dense])
-        _ck(lib().csnet_train_mix_fwd(dst.data_ptr(), n, out_c, out_h, out_w, arr, len(dense), st), "csnet_train_mix_fwd")
+        if bf:
+            _ck(lib().csnet_train_mix_fwd_bf16(dst.data_ptr(), _code(odt), n, out_c, out_h, out_w, arr, len(dense), _code(sdt), st),
+                "csnet_train_mix_fwd_bf16")
+        else:
+            _ck(lib().csnet_train_mix_fwd(dst.data_ptr(), n, out_c, out_h, out_w, arr, len(dense), st), "csnet_train_mix_fwd")
         # a source used only through its pooled copy is not kept
         direct = {p.src for k, p in enumerate(paths) if k not in pooled}
         shapes = [tuple(t.shape) for t in tensors]
@@ -150,14 +221,16 @@ class MixFn(torch.autograd.Function):
             if k in pooled and p.src not in direct:
                 saved[p.src] = None
         ctx.spec, ctx.dense, ctx.pooled, ctx.shapes, ctx.n_in = spec, dense, pooled, shapes, len(tensors)
+        ctx.sdt, ctx.bf = sdt, bf
         ctx.save_for_backward(*saved)
         return dst
 
     @staticmethod
     def backward(ctx, ddst):
-        out_c, out_h, out_w, paths = ctx.spec
+        out_c, out_h, out_w, paths = ctx.spec[:4]
         saved = ctx.saved_tensors
-        ddst = _f32(ddst)
+        sdt, bf = ctx.sdt, ctx.bf
+        ddst = _act(ddst) if bf else _f32(ddst)
         n = ddst.shape[0]
         grads: List[Optional[torch.Tensor]] = [None] * ctx.n_in
         st = _stream(ddst)
@@ -166,22 +239,31 @@ class MixFn(torch.autograd.Function):
             shp = ctx.shapes[p.src]
             if ctx.needs_input_grad[1 + p.src]:
                 xs = saved[q.src].shape
-                d = torch.empty((n, p.cin, xs[2], xs[3]), dtype=torch.float32, device=ddst.device)
-                _ck(lib().csnet_train_mix_dgrad(ddst.data_ptr(), n, out_c, out_h, out_w, C.byref(cp), d.data_ptr(), st), "csnet_train_mix_dgrad")
+                d = torch.empty((n, p.cin, xs[2], xs[3]), dtype=sdt, device=ddst.device)
+                if bf:
+                    _ck(lib().csnet_train_mix_dgrad_bf16(ddst.data_ptr(), _code(ddst.dtype), n, out_c, out_h, out_w, C.byref(cp), d.data_ptr(),
+                                                         _code(sdt), st), "csnet_train_mix_dgrad_bf16")
+                else:
+                    _ck(lib().csnet_train_mix_dgrad(ddst.data_ptr(), n, out_c, out_h, out_w, C.byref(cp), d.data_ptr(), st), "csnet_train_mix_dgrad")
                 if k in ctx.pooled:
                     idx = saved[ctx.pooled[k][1]]
-                    full = torch.empty((n, p.cin, shp[2], shp[3]), dtype=torch.float32, device=ddst.device)
-                    _ck(lib().csnet_train_pool_bwd(d.data_ptr(), idx.data_ptr() if idx is not None else None, n, p.cin, shp[2], shp[3],
-                                                   p.pre_avg, p.pool, full.data_ptr(), st), "csnet_train_pool_bwd")
+                    full = torch.empty((n, p.cin, shp[2], shp[3]), dtype=sdt, device=ddst.device)
+                    fn = "csnet_train_pool_bwd_bf16" if sdt == torch.bfloat16 else "csnet_train_pool_bwd"
+                    _ck(getattr(lib(), fn)(d.data_ptr(), idx.data_ptr() if idx is not None else None, n, p.cin, shp[2], shp[3],
+                                           p.pre_avg, p.pool, full.data_ptr(), st), fn)
                     d = full
                 if p.c0 != 0 or p.cin != shp[1]:
-                    full = torch.zeros(shp, dtype=torch.float32, device=ddst.device)
+                    full = torch.zeros(shp, dtype=sdt, device=ddst.device)
                     full[:, p.c0:p.c0 + p.cin] = d
                     d = full
                 grads[p.src] = d if grads[p.src] is None else grads[p.src] + d
             if p.w is not None and ctx.needs_input_grad[1 + p.w]:
                 dw = torch.empty_like(saved[p.w])
-                _ck(lib().csnet_train_mix_wgrad(ddst.data_ptr(), n, out_c, out_h, out_w, C.byref(cp), dw.data_ptr(), st), "csnet_train_mix_wgrad")
+                if bf:
+                    _ck(lib().csnet_train_mix_wgrad_bf16(ddst.data_ptr(), _code(ddst.dtype), n, out_c, out_h, out_w, C.byref(cp), dw.data_ptr(),
+                                                         _code(sdt), st), "csnet_train_mix_wgrad_bf16")
+                else:
+                    _ck(lib().csnet_train_mix_wgrad(ddst.data_ptr(), n, out_c, out_h, out_w, C.byref(cp), dw.data_ptr(), st), "csnet_train_mix_wgrad")
                 grads[p.w] = dw if grads[p.w] is None else grads[p.w] + dw
         return (None, *grads)
 
@@ -200,7 +282,8 @@ class BnPreluFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, z, gamma, beta, slope, frozen_mean=None, frozen_var=None):
-        z = _f32(z)
+        z = _act(z)                                      # y, dz: z's dtype; statistics, gap and the parameter gradients: fp32
+        sfx = "_bf16" if z.dtype == torch.bfloat16 else ""
         n, c, h, w = z.shape
         y = torch.empty_like(z)
         gap = torch.empty((n, c), dtype=torch.float32, device=z.device)
@@ -212,9 +295,11 @@ class BnPreluFn(torch.autograd.Function):
         else:
             mean = torch.empty(c, dtype=torch.float32, device=z.device)
             var = torch.empty_like(mean)
-            _ck(lib().csnet_train_bn_stats(z.data_ptr(), n, c, h * w, mean.data_ptr(), var.data_ptr(), st), "csnet_train_bn_stats")
-        _ck(lib().csnet_train_bn_prelu_fwd(z.data_ptr(), y.data_ptr(), n, c, h * w, mean.data_ptr(), var.data_ptr(), g.data_ptr(),
-                                           b.data_ptr(), a.data_ptr(), BN_EPS, gap.data_ptr(), st), "csnet_train_bn_prelu_fwd")
+            _ck(getattr(lib(), "csnet_train_bn_stats" + sfx)(z.data_ptr(), n, c, h * w, mean.data_ptr(), var.data_ptr(), st),
+                "csnet_train_bn_stats" + sfx)
+        _ck(getattr(lib(), "csnet_train_bn_prelu_fwd" + sfx)(z.data_ptr(), y.data_ptr(), n, c, h * w, mean.data_ptr(), var.data_ptr(),
+                                                             g.data_ptr(), b.data_ptr(), a.data_ptr(), BN_EPS, gap.data_ptr(), st),
+            "csnet_train_bn_prelu_fwd" + sfx)
         ctx.save_for_backward(z, mean, var, g, b, a)
         ctx.mark_non_differentiable(mean, var, gap)
         return y, mean, var, gap
@@ -222,13 +307,15 @@ class BnPreluFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy, _dm, _dv, _dg):
         z, mean, var, g, b, a = ctx.saved_tensors
-        dy = _f32(dy)
+        bf = z.dtype == torch.bfloat16
+        dy = _act(dy) if bf else _f32(dy)
+        fn = "csnet_train_bn_prelu_bwd_bf16" if bf else "csnet_train_bn_prelu_bwd"
         n, c, h, w = z.shape
         dz = torch.empty_like(z)
         dgamma, dbeta, dslope = (torch.empty(c, dtype=torch.float32, device=z.device) for _ in range(3))
-        _ck(lib().csnet_train_bn_prelu_bwd(z.data_ptr(), dy.data_ptr(), dz.data_ptr(), n, c, h * w, mean.data_ptr(), var.data_ptr(),
-                                           g.data_ptr(), b.data_ptr(), a.data_ptr(), BN_EPS, dgamma.data_ptr(), dbeta.data_ptr(),
-                                           dslope.data_ptr(), int(ctx.frozen), _stream(z)), "csnet_train_bn_prelu_bwd")
+        _ck(getattr(lib(), fn)(z.data_ptr(), dy.data_ptr(), dz.data_ptr(), n, c, h * w, mean.data_ptr(), var.data_ptr(),
+                               g.data_ptr(), b.data_ptr(), a.data_ptr(), BN_EPS, dgamma.data_ptr(), dbeta.data_ptr(),
+                               dslope.data_ptr(), int(ctx.frozen), _stream(z)), fn)
         return dz, dgamma, dbeta, dslope, None, None
 
 
@@ -252,10 +339,12 @@ def bn_prelu_train(z, bn: torch.nn.BatchNorm2d, prelu: torch.nn.PReLU):
 class DwFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w, scale):
-        x, wf = _f32(x), _f32(w.detach()).reshape(-1, 9)
+        x, wf = _act(x), _f32(w.detach()).reshape(-1, 9)       # y, dx: x's dtype; dw: fp32
+        sfx = "_bf16" if x.dtype == torch.bfloat16 else ""
         n, c, h, ww = x.shape
         y = torch.empty_like(x)
-        _ck(lib().csnet_train_dw_conv(x.data_ptr(), wf.data_ptr(), y.data_ptr(), n, c, h, ww, scale, 0, _stream(x)), "csnet_train_dw_conv")
+        _ck(getattr(lib(), "csnet_train_dw_conv" + sfx)(x.data_ptr(), wf.data_ptr(), y.data_ptr(), n, c, h, ww, scale, 0, _stream(x)),
+            "csnet_train_dw_conv" + sfx)
         ctx.save_for_backward(x, wf)
         ctx.scale, ctx.wshape = scale, w.shape
         return y
@@ -263,20 +352,24 @@ class DwFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         x, wf = ctx.saved_tensors
-        dy = _f32(dy)
+        bf = x.dtype == torch.bfloat16
+        sfx = "_bf16" if bf else ""
+        dy = _act(dy) if bf else _f32(dy)
         n, c, h, ww = x.shape
         dx = dw = None
         if ctx.needs_input_grad[0] and ctx.needs_input_grad[1]:          # the usual case: one pass over dy for both gradients
             dx, dw = torch.empty_like(x), torch.empty_like(wf)
-            _ck(lib().csnet_train_dw_bwd(x.data_ptr(), dy.data_ptr(), wf.data_ptr(), dx.data_ptr(), dw.data_ptr(), n, c, h, ww, ctx.scale,
-                                         _stream(x)), "csnet_train_dw_bwd")
+            _ck(getattr(lib(), "csnet_train_dw_bwd" + sfx)(x.data_ptr(), dy.data_ptr(), wf.data_ptr(), dx.data_ptr(), dw.data_ptr(), n, c, h, ww,
+                                                           ctx.scale, _stream(x)), "csnet_train_dw_bwd" + sfx)
             return dx, dw.reshape(ctx.wshape), None
         if ctx.needs_input_grad[0]:
             dx = torch.empty_like(x)
-            _ck(lib().csnet_train_dw_conv(dy.data_ptr(), wf.data_ptr(), dx.data_ptr(), n, c, h, ww, ctx.scale, 1, _stream(x)), "csnet_train_dw_conv(T)")
+            _ck(getattr(lib(), "csnet_train_dw_conv" + sfx)(dy.data_ptr(), wf.data_ptr(), dx.data_ptr(), n, c, h, ww, ctx.scale, 1, _stream(x)),
+                "csnet_train_dw_conv" + sfx + "(T)")
         if ctx.needs_input_grad[1]:
             dw = torch.empty_like(wf)
-            _ck(lib().csnet_train_dw_wgrad(x.data_ptr(), dy.data_ptr(), dw.data_ptr(), n, c, h, ww, ctx.scale, _stream(x)), "csnet_train_dw_wgrad")
+            _ck(getattr(lib(), "csnet_train_dw_wgrad" + sfx)(x.data_ptr(), dy.data_ptr(), dw.data_ptr(), n, c, h, ww, ctx.scale, _stream(x)),
+                "csnet_train_dw_wgrad" + sfx)
             dw = dw.reshape(ctx.wshape)
         return dx, dw, None
 

@@ -64,9 +64,13 @@ class FlatGrads:
 
 class Trainer:
     def __init__(self, model, lr: float = 1e-4, weight_decay: float = 5e-3, betas=(0.9, 0.99), eps: float = 1e-8,
-                 flops_weight: Optional[float] = None, flops_expand: float = 1.0, process_group=None, recompute: bool = False):
+                 flops_weight: Optional[float] = None, flops_expand: float = 1.0, process_group=None, recompute: bool = False,
+                 storage: str = "fp32"):
+        if storage not in T.STORAGES:
+            raise ValueError(f"storage must be one of {sorted(T.STORAGES)}, got {storage!r}")
         self.model = model
         model.recompute = bool(recompute)        # modular.csnet_forward: checkpoint every ILBlock (memory for one extra forward)
+        model.train_storage = storage            # modular.csnet_forward: activation storage, "fp32" or "bf16" (DESIGN.md §6)
         self.flops_weight = flops_weight
         self.group = process_group
         if flops_weight is not None:
