@@ -205,16 +205,15 @@ __device__ __forceinline__ void dw_task(int task, const uint16_t* in, uint16_t* 
   const int gi = task % G, rest = task / G;
   const int run = rest % NR, c = rest / NR;
   const int x = 4 * (GEO::G0 + gi), ra = GEO::R0 + run * RUN;
-  // fp16 planes: the 9 taps run as Pack<T>::fma16 (16-bit x 16-bit + fp32, one rounding) with the weights packed as
-  // fp16 pairs, which halves their registers (measured: no change of the fp16 error figures).
-  // bf16 planes keep fp32 weights and converted operands — 8-bit-mantissa weights cost accuracy there.
+  // fp16 planes: the row window is converted to fp32 once and the weights are the fp32 values of their fp16 rounding, so
+  // each of the 9 taps is one FFMA with the product of a 16-bit x 16-bit + fp32 FMA (measured: no change of the fp16 error
+  // figures).  bf16 planes keep fp32 weights and convert the operand per tap — 8-bit-mantissa weights cost accuracy there.
   constexpr bool kMixed = std::is_same<T, __half>::value;
   float wf[9];
-  uint16_t wh[9];
 #pragma unroll
   for (int i = 0; i < 9; ++i) {
     wf[i] = __ldg(P.w + c * 9 + i);
-    wh[i] = Pack<T>::bits(wf[i]);
+    if constexpr (kMixed) wf[i] = Pack<T>::to_f(Pack<T>::bits(wf[i]));
   }
   const float bias = __ldg(P.b + c), slope_m1 = __ldg(P.s + c) - 1.f;
   const uint16_t* plane = in + c * NP + x;
@@ -234,6 +233,11 @@ __device__ __forceinline__ void dw_task(int task, const uint16_t* in, uint16_t* 
     rows[i][0] = (uint16_t)(lft >> 16); rows[i][1] = (uint16_t)mid.x; rows[i][2] = (uint16_t)(mid.x >> 16);
     rows[i][3] = (uint16_t)mid.y; rows[i][4] = (uint16_t)(mid.y >> 16); rows[i][5] = (uint16_t)rgt;
   }
+  float rowf[RUN + 2][6];                              // fp16 only
+#pragma unroll
+  for (int i = 0; i < RUN + 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 6; ++j) rowf[i][j] = Pack<T>::to_f(rows[i][j]);
 #pragma unroll
   for (int i = 0; i < RUN; ++i) {
     const int r = ra + i;
@@ -246,7 +250,7 @@ __device__ __forceinline__ void dw_task(int task, const uint16_t* in, uint16_t* 
         for (int dy = 0; dy < 3; ++dy)
 #pragma unroll
           for (int dx = 0; dx < 3; ++dx) {
-            if constexpr (kMixed) v = Pack<T>::fma16(rows[i + dy][k + dx], wh[dy * 3 + dx], v);
+            if constexpr (kMixed) v = fmaf(rowf[i + dy][k + dx], wf[dy * 3 + dx], v);
             else v = fmaf(Pack<T>::to_f(rows[i + dy][k + dx]), wf[dy * 3 + dx], v);
           }
         o[k] = prelu_m1(v, slope_m1);

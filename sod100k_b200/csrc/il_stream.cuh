@@ -191,9 +191,6 @@ __device__ __forceinline__ void sts128(uint32_t a, uint4 v) {
 }
 __device__ __forceinline__ void sts16(uint32_t a, uint16_t v) { asm volatile("st.shared.u16 [%0], %1;\n" ::"r"(a), "h"(v) : "memory"); }
 
-// element j of a row of packed 16-bit pairs
-__device__ __forceinline__ uint16_t h16(const uint32_t* row, int j) { return (j & 1) ? (uint16_t)(row[j >> 1] >> 16) : (uint16_t)row[j >> 1]; }
-
 // The depthwise tail.  A thread owns one channel and two 8-pixel groups A, B (x0 .. x0+15) of a strip row for the whole
 // walk and keeps running sums instead of windows of its inputs: a 3x3 output row is finished by its third input row, so per
 // layer the thread holds the two output rows still open (one started by one input row, one by two).  Each input value is

@@ -2,8 +2,10 @@
 // PReLU) on 16-bit activations: few output channels (1..8 per dilation), so it is a depthwise-like problem for the FP32 pipe,
 // not for the tensor cores.  A thread owns PX output pixels of one row for all of the path's output channels; per (input
 // channel, tap row) it loads the needed 8-pixel groups once (16-byte read-only loads, L1-resident across the taps and the
-// neighbouring rows) and feeds them to the mixed-precision FMA (fp16 x fp16 + fp32, no conversions): the half-word select of
-// the instruction resolves odd pixel shifts for free.  The dilation is a template parameter, so every register index is static.
+// neighbouring rows), one row ahead of its FMAs, and converts the pixels the taps read to fp32 once.  The weights sit in
+// shared memory as the fp32 values of their 16-bit rounding, so every tap is one FFMA on registers and a broadcast shared
+// load: the products and their order (ci, ky, kx) are those of a 16-bit x 16-bit + fp32 FMA.  The dilation is a template
+// parameter, so every register index is static.
 #pragma once
 #include "il_stream.cuh"
 
@@ -32,11 +34,12 @@ template <int D, int PX> struct MsdGeom {
 template <typename T, int D, int PX, int COMAX>
 __global__ void __launch_bounds__(kMsdThreads) msd_kernel(const __grid_constant__ MsdArgs A) {
   using GEO = MsdGeom<D, PX>;
-  extern __shared__ __align__(16) uint16_t sw[];                          // [cin][9][COMAX] 16-bit weights
+  static_assert(COMAX % 2 == 0, "weights are read as fp32 pairs");
+  extern __shared__ __align__(16) float sw[];                             // [cin][9][COMAX] fp32 values of the 16-bit weights
   const int tid = threadIdx.x;
   for (int i = tid; i < A.Cin * 9 * COMAX; i += kMsdThreads) {
     const int co = i % COMAX, ct = i / COMAX;
-    sw[i] = co < A.cout ? Pack<T>::bits(__ldg(A.w + (size_t)ct * A.cout + co)) : (uint16_t)0;
+    sw[i] = co < A.cout ? Pack<T>::to_f(Pack<T>::bits(__ldg(A.w + (size_t)ct * A.cout + co))) : 0.f;
   }
   __syncthreads();
   const int strips = A.W / PX;
@@ -55,40 +58,62 @@ __global__ void __launch_bounds__(kMsdThreads) msd_kernel(const __grid_constant_
     const int gx = x0 + GEO::kFirst + g * GEO::kStep;
     gin[g] = gx >= 0 && gx < W;
   }
-  const uint16_t* img = A.src + (size_t)n * A.Cin * H * W + x0 + GEO::kFirst;
-  for (int ci = 0; ci < A.Cin; ++ci, img += (size_t)H * W) {
+  const size_t plane = (size_t)H * W;
+  const uint16_t* img = A.src + (size_t)n * A.Cin * plane + x0 + GEO::kFirst;
+  bool rin[3];                                                             // tap row inside the image? (else zero padding)
+#pragma unroll
+  for (int ky = 0; ky < 3; ++ky) rin[ky] = y + D * (ky - 1) >= 0 && y + D * (ky - 1) < H;
+  // software pipeline over the (ci, ky) rows: the groups of the next row are in flight while this row's FMAs run; a row
+  // outside the image is not read
+  uint4 cur[GEO::kGroups];
+#pragma unroll
+  for (int g = 0; g < GEO::kGroups; ++g)
+    cur[g] = rin[0] && gin[g] ? __ldg(reinterpret_cast<const uint4*>(img + (ptrdiff_t)(y - D) * W + g * GEO::kStep))
+                              : make_uint4(0u, 0u, 0u, 0u);
+  for (int ci = 0; ci < A.Cin; ++ci, img += plane) {
 #pragma unroll
     for (int ky = 0; ky < 3; ++ky) {
-      const int r = y + D * (ky - 1);
-      if (r < 0 || r >= H) continue;                                       // zero padding rows
-      const uint16_t* row = img + (size_t)r * W;
-      uint32_t win[GEO::kGroups][4];
+      const int kn = ky < 2 ? ky + 1 : 0;                                  // next row: (ci, ky + 1) or (ci + 1, 0)
+      const uint16_t* next = (ky < 2 ? img : img + plane) + (ptrdiff_t)(y + D * (kn - 1)) * W;
+      const bool nin = rin[kn] && (ky < 2 || ci + 1 < A.Cin);
+      uint4 nxt[GEO::kGroups];
 #pragma unroll
-      for (int g = 0; g < GEO::kGroups; ++g) {
-        uint4 v = make_uint4(0u, 0u, 0u, 0u);
-        if (gin[g]) v = __ldg(reinterpret_cast<const uint4*>(row + g * GEO::kStep));
-        win[g][0] = v.x; win[g][1] = v.y; win[g][2] = v.z; win[g][3] = v.w;
-      }
-      const uint16_t* wrow = sw + (ci * 9 + ky * 3) * COMAX;
+      for (int g = 0; g < GEO::kGroups; ++g)
+        nxt[g] = nin && gin[g] ? __ldg(reinterpret_cast<const uint4*>(next + g * GEO::kStep)) : make_uint4(0u, 0u, 0u, 0u);
+      if (rin[ky]) {
+        float xf[GEO::kGroups * 8];                                          // pixels no tap reads are never converted
 #pragma unroll
-      for (int kx = 0; kx < 3; ++kx) {
-        uint32_t wreg[(COMAX + 1) / 2];
+        for (int g = 0; g < GEO::kGroups; ++g) {
+          const uint32_t u[4] = {cur[g].x, cur[g].y, cur[g].z, cur[g].w};
 #pragma unroll
-        for (int j = 0; j < (COMAX + 1) / 2; ++j)
-          wreg[j] = COMAX == 1 ? (uint32_t)wrow[kx] : reinterpret_cast<const uint32_t*>(wrow + kx * COMAX)[j];
+          for (int j = 0; j < 4; ++j) {
+            const float2 f = Pack<T>::to_f2(u[j]);
+            xf[g * 8 + 2 * j] = f.x; xf[g * 8 + 2 * j + 1] = f.y;
+          }
+        }
+        const float* wrow = sw + (ci * 9 + ky * 3) * COMAX;
 #pragma unroll
-        for (int co = 0; co < COMAX; ++co) {
-          if (co < A.cout) {                                               // uniform
-            const uint16_t wv = h16(wreg, co);
+        for (int kx = 0; kx < 3; ++kx) {
+          float wk[COMAX];
 #pragma unroll
-            for (int p = 0; p < PX; ++p) {
-              constexpr int dummy = 0; (void)dummy;
-              const int i = p + D * (kx - 1);                              // static after unrolling
-              acc[co][p] = Pack<T>::fma16(h16(win[GEO::grp(i)], GEO::pix(i)), wv, acc[co][p]);
+          for (int j = 0; j < COMAX; j += 2) {
+            const float2 w2 = reinterpret_cast<const float2*>(wrow + kx * COMAX)[j / 2];
+            wk[j] = w2.x; wk[j + 1] = w2.y;
+          }
+#pragma unroll
+          for (int co = 0; co < COMAX; ++co) {
+            if (co < A.cout) {                                               // uniform
+#pragma unroll
+              for (int p = 0; p < PX; ++p) {
+                const int i = p + D * (kx - 1);                              // static after unrolling
+                acc[co][p] = fmaf(xf[GEO::grp(i) * 8 + GEO::pix(i)], wk[co], acc[co][p]);
+              }
             }
           }
         }
       }
+#pragma unroll
+      for (int g = 0; g < GEO::kGroups; ++g) cur[g] = nxt[g];
     }
   }
   uint16_t* out = A.dst + (((size_t)n * A.Ctot + A.cout0) * H + y) * W + x0;
@@ -113,7 +138,7 @@ template <typename T, int PX, int COMAX>
 inline void msd_launch_d(int dil, const MsdArgs& A, cudaStream_t st) {
   const long long tasks = (long long)A.N * A.H * (A.W / PX);
   const unsigned grid = (unsigned)((tasks + kMsdThreads - 1) / kMsdThreads);
-  const size_t smem = (size_t)A.Cin * 9 * COMAX * 2;
+  const size_t smem = (size_t)A.Cin * 9 * COMAX * sizeof(float);
   switch (dil) {
     case 1: msd_kernel<T, 1, PX, COMAX><<<grid, kMsdThreads, smem, st>>>(A); break;
     case 2: msd_kernel<T, 2, PX, COMAX><<<grid, kMsdThreads, smem, st>>>(A); break;
