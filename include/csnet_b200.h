@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define CSNET_ABI_VERSION 13
+#define CSNET_ABI_VERSION 14
 
 enum { CSNET_F32 = 0, CSNET_F16 = 1, CSNET_BF16 = 2 };
 
@@ -473,6 +473,50 @@ int csnet_train_resize_fwd(const float* src, int32_t N, int32_t C, int32_t Hs, i
                            int32_t accumulate, void* stream);
 int csnet_train_resize_bwd(const float* ddst, int32_t N, int32_t C, int32_t Hd, int32_t Wd, float* dsrc, int32_t Hs, int32_t Ws,
                            void* stream);
+
+/* ---- CSF+Res2Net head training with bf16 activation storage (sod100k_b200/modular_r.py picks these when net.train_storage is
+ * "bf16") ----------------------------------------------------------------------------------------------------------------------
+ * The calls above on bf16 planar NCHW activations and activation gradients (pointers are void*).  Convolutions run on a tensor-core
+ * implicit GEMM (csrc/gemm_bf16.cuh: mma.sync bf16 x bf16 -> fp32, 128 x 128 x 32 block tiles): operands bf16, accumulation fp32,
+ * the weights the fp32 parameters rounded to nearest-even bf16 (csnet_train_cast_bf16).  Forward and data-gradient destinations are
+ * bf16 or fp32 (dst_dtype / dsrc_dtype: CSNET_BF16 or CSNET_F32); weight gradients, bias, GroupNorm statistics, gamma / beta / slope and
+ * their gradients stay fp32.  Every bf16 store is rounded once to nearest even; split-K partials are merged in split order and
+ * reductions keep the fp32 calls' order (no floating-point atomics: the same bits on every run).  Segments, splits and workspace
+ * are as for csnet_train_conv_*; there is one block tile, so no tile argument. */
+typedef struct {
+  const void* src;        /* bf16 [N, C, H, W]: fwd / wgrad the conv's input, dgrad the gradient of the conv's output tensor */
+  const void* w;          /* bf16 weight slice (unused by wgrad, which writes the fp32 gradient at the same layout) */
+  int32_t C, c0, cin;
+  int32_t cout0, cout;
+  int32_t ksize, dil, ldw;
+} csnet_conv_seg_bf16;    /* 48 bytes, csnet_conv_seg's layout */
+
+/* dst[i] = bf16 nearest-even rounding of src[i], i < n (the weights of a step, rounded once) */
+int csnet_train_cast_bf16(const float* src, void* dst, int64_t n, void* stream);
+/* splits, the k extent of one split (chain) and the workspace bytes of a conv call, arguments as the call's */
+int csnet_train_conv_plan_bf16(int32_t form, int32_t N, int32_t H, int32_t W, const csnet_conv_seg_bf16* segs, int32_t n_segs,
+                               int32_t splits, int32_t* splits_out, int32_t* chain_out, int64_t* ws_bytes);
+int csnet_train_conv_fwd_bf16(void* dst, int32_t dst_dtype, int32_t N, int32_t C, int32_t H, int32_t W, const csnet_conv_seg_bf16* segs,
+                              int32_t n_segs, const float* bias, int32_t accumulate, int32_t splits, float* ws, int64_t ws_bytes,
+                              void* stream);
+int csnet_train_conv_dgrad_bf16(void* dsrc, int32_t dsrc_dtype, int32_t N, int32_t C, int32_t H, int32_t W, int32_t c0, int32_t cin,
+                                const csnet_conv_seg_bf16* segs, int32_t n_segs, int32_t accumulate, int32_t splits, float* ws,
+                                int64_t ws_bytes, void* stream);
+/* ddst bf16; dw fp32 */
+int csnet_train_conv_wgrad_bf16(const void* ddst, int32_t N, int32_t Cd, int32_t H, int32_t W, const csnet_conv_seg_bf16* seg, float* dw,
+                                int32_t accumulate, int32_t splits, float* ws, int64_t ws_bytes, void* stream);
+/* z, y, dy, dz bf16; mean / var / ws and the parameter gradients fp32 */
+int csnet_train_gn_stats_bf16(const void* z, int32_t N, int32_t C, int32_t HW, int32_t groups, float* mean, float* var, void* stream);
+int csnet_train_gn_prelu_fwd_bf16(const void* z, void* y, int32_t N, int32_t C, int32_t HW, int32_t groups, const float* mean,
+                                  const float* var, const float* gamma, const float* beta, const float* slope, float eps, void* stream);
+int csnet_train_gn_prelu_bwd_bf16(const void* z, const void* dy, void* dz, int32_t N, int32_t C, int32_t HW, int32_t groups,
+                                  const float* mean, const float* var, const float* gamma, const float* beta, const float* slope, float eps,
+                                  float* dgamma, float* dbeta, float* dslope, float* ws, void* stream);
+/* bf16 on both sides; the adjoint sums in fp32 over the same taps as csnet_train_resize_bwd */
+int csnet_train_resize_fwd_bf16(const void* src, int32_t N, int32_t C, int32_t Hs, int32_t Ws, void* dst, int32_t Hd, int32_t Wd,
+                                int32_t accumulate, void* stream);
+int csnet_train_resize_bwd_bf16(const void* ddst, int32_t N, int32_t C, int32_t Hd, int32_t Wd, void* dsrc, int32_t Hs, int32_t Ws,
+                                void* stream);
 
 /* ---- evaluation: the counting part of SalMetric on the device (CSNet_training/SalMetric/src/sal_metric.cpp:86-120) ----
  * prob: device float32 [N][HW] saliency in [0,1] (after sigmoid); gt: device uint8 [N][HW] ground truth.  Per image:

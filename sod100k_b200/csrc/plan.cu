@@ -1410,6 +1410,57 @@ int csnet_train_resize_bwd(const float* ddst, int32_t N, int32_t C, int32_t Hd, 
   return CSNET_OK;
 }
 
+}  // extern "C"
+
+// The same pair on bf16 activations (CSF+Res2Net training with bf16 storage): resize_kernel<bf16, bf16>, and the adjoint's gather on
+// bf16 gradients (fp32 sums over the same taps, rounded once to bf16).
+namespace {
+__global__ void __launch_bounds__(csnet::kRzAdjThreads) resize_bwd_bf16_kernel(const __nv_bfloat16* __restrict__ ddst,
+                                                                        __nv_bfloat16* __restrict__ dsrc, int C, int Hs, int Ws, int Hd,
+                                                                        int Wd, float sy, float sx) {
+  const int p = blockIdx.x * csnet::kRzAdjThreads + threadIdx.x;
+  if (p >= Hs * Ws) return;
+  const int c = blockIdx.y, n = blockIdx.z, ys = p / Ws, xs = p - ys * Ws;
+  const __nv_bfloat16* g = ddst + ((int64_t)n * C + c) * Hd * Wd;
+  dsrc[((int64_t)n * C + c) * Hs * Ws + p] = __float2bfloat16_rn(csnet::resize_adj_value(g, Hs, Ws, Hd, Wd, sy, sx, ys, xs));
+}
+}  // namespace
+
+extern "C" {
+
+
+int csnet_train_resize_fwd_bf16(const void* src, int32_t N, int32_t C, int32_t Hs, int32_t Ws, void* dst, int32_t Hd, int32_t Wd,
+                                int32_t accumulate, void* stream) {
+  if (!src || !dst || N < 1 || N > 65535 || C < 1 || C > 8 * 65535 || Hs < 1 || Ws < 1 || Hd < 1 || Wd < 1) {
+    csnet::train_set_error("csnet_train_resize_fwd_bf16: bad arguments");
+    return CSNET_E_INVALID;
+  }
+  csnet::RzArgs A{};
+  A.src = src; A.dst = dst;
+  A.Cs = C; A.Hs = Hs; A.Ws = Ws; A.c0 = 0;
+  A.Cd = C; A.Hd = Hd; A.Wd = Wd; A.cout0 = 0;
+  A.C = C; A.accumulate = accumulate != 0;
+  A.sy = csnet::resize_scale(Hs, Hd); A.sx = csnet::resize_scale(Ws, Wd);
+  csnet::launch_resize(A, CSNET_BF16, CSNET_BF16, N, (cudaStream_t)stream);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { csnet::train_set_error(cudaGetErrorString(e)); return CSNET_E_CUDA; }
+  return CSNET_OK;
+}
+
+int csnet_train_resize_bwd_bf16(const void* ddst, int32_t N, int32_t C, int32_t Hd, int32_t Wd, void* dsrc, int32_t Hs, int32_t Ws,
+                                void* stream) {
+  if (!ddst || !dsrc || N < 1 || N > 65535 || C < 1 || C > 65535 || Hs < 1 || Ws < 1 || Hd < 1 || Wd < 1 || (int64_t)Hs * Ws > (1 << 30)) {
+    csnet::train_set_error("csnet_train_resize_bwd_bf16: bad arguments");
+    return CSNET_E_INVALID;
+  }
+  const dim3 grid((unsigned)((Hs * Ws + csnet::kRzAdjThreads - 1) / csnet::kRzAdjThreads), (unsigned)C, (unsigned)N);
+  resize_bwd_bf16_kernel<<<grid, csnet::kRzAdjThreads, 0, (cudaStream_t)stream>>>(
+      (const __nv_bfloat16*)ddst, (__nv_bfloat16*)dsrc, C, Hs, Ws, Hd, Wd, csnet::resize_scale(Hs, Hd), csnet::resize_scale(Ws, Wd));
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) { csnet::train_set_error(cudaGetErrorString(e)); return CSNET_E_CUDA; }
+  return CSNET_OK;
+}
+
 int csnet_salmetric_images_u8(const float* logits, int32_t N, int32_t H, int32_t W, const csnet_image_geom* geom, const uint8_t* m_packed,
                               uint8_t* y_packed, uint32_t* hist_all, uint32_t* hist_pos, unsigned long long* abs_sum, void* stream) {
   if (!logits || !geom || !m_packed || !hist_all || !hist_pos || !abs_sum)

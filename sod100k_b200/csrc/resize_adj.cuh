@@ -40,15 +40,16 @@ CSNET_IO_HD RzRange rz_src_range(int s, int n_in, int n_out, float scale) {
 // Weight output o gives source s along one axis.
 CSNET_IO_HD float rz_adj_weight(MaeTap t, int s) { return (t.i0 == s ? t.l0 : 0.f) + (t.i1 == s ? t.l1 : 0.f); }
 
-// One source value of the adjoint: g = the output-gradient channel [Hd][Wd].
-CSNET_IO_HD float resize_adj_value(const float* g, int Hs, int Ws, int Hd, int Wd, float sy, float sx, int ys, int xs) {
+// One source value of the adjoint: g = the output-gradient channel [Hd][Wd] (fp32, or bf16 widened exactly; the sums are fp32).
+template <typename T>
+CSNET_IO_HD float resize_adj_value(const T* g, int Hs, int Ws, int Hd, int Wd, float sy, float sx, int ys, int xs) {
   const RzRange ry = rz_src_range(ys, Hs, Hd, sy), rx = rz_src_range(xs, Ws, Wd, sx);
   float acc = 0.f;
   for (int oy = ry.lo; oy <= ry.hi; ++oy) {
     const float wy = rz_adj_weight(mae_tap(oy, Hs, sy), ys);
-    const float* row = g + (int64_t)oy * Wd;
+    const T* row = g + (int64_t)oy * Wd;
     float r = 0.f;
-    for (int ox = rx.lo; ox <= rx.hi; ++ox) r += rz_adj_weight(mae_tap(ox, Ws, sx), xs) * row[ox];
+    for (int ox = rx.lo; ox <= rx.hi; ++ox) r += rz_adj_weight(mae_tap(ox, Ws, sx), xs) * rz_f32(row[ox]);
     acc += wy * r;
   }
   return acc;

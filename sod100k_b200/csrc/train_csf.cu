@@ -1,4 +1,5 @@
-// train_csf.cu — training kernels of the CSF+Res2Net head (fp32), C ABI csnet_train_conv_* / _bias_grad / _gn_* (include/csnet_b200.h).
+// train_csf.cu — training kernels of the CSF+Res2Net head (fp32), C ABI csnet_train_conv_* / _bias_grad / _gn_* (include/csnet_b200.h), and the
+// bf16-storage twins of the _gn_* calls (the bf16 convolutions are in train_csf_bf16.cu).
 //
 // The head (fuse, ms, fuse1x1, cls_layer: networks/gOctConv.py, csf_res2net.py) is 1x1 and dilated 3x3 convolutions with K = 128..3840
 // and N = 128..1408 channels, GroupNorm(32) + PReLU, and bilinear resizes between the Res2Net stages.  The convolutions run on the fp32
@@ -10,6 +11,7 @@
 
 #include "../../include/csnet_b200.h"
 #include "gemm_f32.cuh"
+#include "gn_bf16.cuh"
 #include "gn_train.cuh"
 
 namespace csnet {
@@ -237,6 +239,40 @@ int csnet_train_gn_prelu_bwd(const float* z, const float* dy, float* dz, int32_t
   CF_CHECK(cudaGetLastError());
   csnet::gn::gn_bwd_dz_kernel<<<dim3(C, N), csnet::gn::kThreads, 0, st>>>(z, dy, dz, N, C, HW, groups, mean, var, gamma, beta, slope, eps,
                                                                          ws, dgamma, dbeta, dslope);
+  CF_CHECK(cudaGetLastError());
+  return 0;
+}
+
+// The same calls on bf16 z / y / dy / dz (CSF+Res2Net training with bf16 storage).
+int csnet_train_gn_stats_bf16(const void* z, int32_t N, int32_t C, int32_t HW, int32_t groups, float* mean, float* var, void* stream) {
+  if (!z || !mean || !var || !gn_args_ok(N, C, HW, groups)) return cfail(CSNET_E_INVALID, "gn_stats_bf16: bad arguments");
+  csnet::gn::gn_stats_bf16_kernel<<<N * groups, csnet::gn::kStatThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)z, C, HW, groups, mean, var);
+  CF_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int csnet_train_gn_prelu_fwd_bf16(const void* z, void* y, int32_t N, int32_t C, int32_t HW, int32_t groups, const float* mean,
+                                  const float* var, const float* gamma, const float* beta, const float* slope, float eps, void* stream) {
+  if (!z || !y || !mean || !var || !gamma || !beta || !slope || !gn_args_ok(N, C, HW, groups))
+    return cfail(CSNET_E_INVALID, "gn_prelu_fwd_bf16: bad arguments");
+  csnet::gn::gn_prelu_fwd_bf16_kernel<<<dim3(C, N), csnet::gn::kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)z, (__nv_bfloat16*)y, C, HW, groups, mean, var, gamma,
+                                                                              beta, slope, eps);
+  CF_CHECK(cudaGetLastError());
+  return 0;
+}
+
+int csnet_train_gn_prelu_bwd_bf16(const void* z, const void* dy, void* dz, int32_t N, int32_t C, int32_t HW, int32_t groups,
+                                  const float* mean, const float* var, const float* gamma, const float* beta, const float* slope, float eps,
+                                  float* dgamma, float* dbeta, float* dslope, float* ws, void* stream) {
+  if (!z || !dy || !dz || !mean || !var || !gamma || !beta || !slope || !dgamma || !dbeta || !dslope || !ws ||
+      !gn_args_ok(N, C, HW, groups))
+    return cfail(CSNET_E_INVALID, "gn_prelu_bwd_bf16: bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  csnet::gn::gn_bwd_reduce_bf16_kernel<<<dim3(C, N), csnet::gn::kThreads, 0, st>>>((const __nv_bfloat16*)z, (const __nv_bfloat16*)dy, C, HW, groups, mean, var, gamma, beta,
+                                                             slope, eps, ws);
+  CF_CHECK(cudaGetLastError());
+  csnet::gn::gn_bwd_dz_bf16_kernel<<<dim3(C, N), csnet::gn::kThreads, 0, st>>>((const __nv_bfloat16*)z, (const __nv_bfloat16*)dy, (__nv_bfloat16*)dz, N, C, HW, groups, mean, var, gamma,
+                                                         beta, slope, eps, ws, dgamma, dbeta, dslope);
   CF_CHECK(cudaGetLastError());
   return 0;
 }

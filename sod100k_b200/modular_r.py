@@ -8,7 +8,13 @@ networks/gOctConv.py:60-114 and csf_res2net.py:205-259:
     resize-added to the sum, in ascending i (the reference's `sum(ysets[j])`).
   * GroupNorm(32) + PReLU per branch; MSBlock's five dilated 3x3 convs write their channel slices of one tensor; cls_layer with
     bias; the final bilinear resize to the input size.
-torch is plumbing here (storage, the tape); every kernel that touches an activation or a gradient is ours, fp32 throughout.
+torch is plumbing here (storage, the tape); every kernel that touches an activation or a gradient is ours.
+
+Activation storage (`net.train_storage`, set by CSFTrainer(storage=...)): "fp32" (default) or "bf16".  Each Function follows the dtype of
+the activations it receives: fp32 runs the fp32 kernels above; bf16 (the backbone's features under autocast) runs their `_bf16` twins,
+with the convolutions on the tensor-core GEMM.  In bf16 the activations and their gradients are bf16; parameters, their gradients,
+GroupNorm statistics, cls_layer's 1-channel map and the logits stay fp32.  A step rounds each weight to bf16 once, in the forward, and
+the data gradient reads the same rounded copy.
 """
 from __future__ import annotations
 
@@ -18,6 +24,7 @@ from typing import List, NamedTuple, Optional, Sequence
 import torch
 
 from . import runtime, splits
+from . import train_ops as T
 
 GN_EPS = 1e-5
 GN_GROUPS = 32
@@ -50,6 +57,16 @@ def lib():
         l.csnet_train_gn_prelu_bwd.argtypes = [vp, vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, f, vp, vp, vp, vp, vp]
         l.csnet_train_resize_fwd.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, i32, vp]
         l.csnet_train_resize_bwd.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, vp]
+        l.csnet_train_cast_bf16.argtypes = [vp, vp, i64, vp]
+        l.csnet_train_conv_plan_bf16.argtypes = [i32, i32, i32, i32, segp, i32, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64)]
+        l.csnet_train_conv_fwd_bf16.argtypes = [vp, i32, i32, i32, i32, i32, segp, i32, vp, i32, i32, vp, i64, vp]
+        l.csnet_train_conv_dgrad_bf16.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, segp, i32, i32, i32, vp, i64, vp]
+        l.csnet_train_conv_wgrad_bf16.argtypes = [vp, i32, i32, i32, i32, segp, vp, i32, i32, vp, i64, vp]
+        l.csnet_train_gn_stats_bf16.argtypes = l.csnet_train_gn_stats.argtypes
+        l.csnet_train_gn_prelu_fwd_bf16.argtypes = l.csnet_train_gn_prelu_fwd.argtypes
+        l.csnet_train_gn_prelu_bwd_bf16.argtypes = l.csnet_train_gn_prelu_bwd.argtypes
+        l.csnet_train_resize_fwd_bf16.argtypes = l.csnet_train_resize_fwd.argtypes
+        l.csnet_train_resize_bwd_bf16.argtypes = l.csnet_train_resize_bwd.argtypes
         _lib = l
     return _lib
 
@@ -71,13 +88,45 @@ def _f32(t: torch.Tensor) -> torch.Tensor:
     return t.contiguous()
 
 
+def _act(t: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+    """An activation or gradient of the given storage dtype, contiguous."""
+    if not t.is_cuda:
+        raise runtime.EngineError("CSF+Res2Net training runs on the GPU only: got a CPU tensor")
+    if t.dtype != dtype:
+        raise runtime.EngineError(f"CSF+Res2Net training with {dtype} storage: got a {t.dtype} activation")
+    return t.contiguous()
+
+
+def _storage(t: torch.Tensor) -> torch.dtype:
+    """The storage dtype a Function runs in: that of the activation it receives."""
+    if t.dtype not in (torch.float32, torch.bfloat16):
+        raise runtime.EngineError(f"CSF+Res2Net training stores fp32 or bf16 activations: got {t.dtype}")
+    return t.dtype
+
+
+def train_dtype(net) -> torch.dtype:
+    """The activation dtype of `net`'s training forward (net.train_storage); any value but "fp32" / "bf16" raises ValueError."""
+    storage = getattr(net, "train_storage", "fp32")
+    if storage not in T.STORAGES:
+        raise ValueError(f"train_storage must be one of {sorted(T.STORAGES)}, got {storage!r}")
+    return T.STORAGES[storage]
+
+
+def cast_bf16(t: torch.Tensor) -> torch.Tensor:
+    """fp32 -> bf16, round to nearest even (csnet_train_cast_bf16)."""
+    t = _f32(t)
+    out = torch.empty(t.shape, dtype=torch.bfloat16, device=t.device)
+    _ck(lib().csnet_train_cast_bf16(t.data_ptr(), out.data_ptr(), t.numel(), _st(t)), "csnet_train_cast_bf16")
+    return out
+
+
 # ---- raw kernel calls ------------------------------------------------------------------------------------------------
 def seg(src: torch.Tensor, w: torch.Tensor, co0: int, co1: int, ci0: int, ci1: int, c0: int = 0, cout0: int = 0, dil: int = 1) -> ConvSeg:
     """Segment of the conv with weight slice w[co0:co1, ci0:ci1] (w: a full OIHW parameter, contiguous).  fwd / wgrad: `src` is the
     input, read from channel c0; dgrad: pass the output's gradient as `src`, its slice starting at cout0."""
     k = w.shape[2]
     ldw = w.shape[1] * k * k
-    wp = w.data_ptr() + 4 * (co0 * ldw + ci0 * k * k)
+    wp = w.data_ptr() + w.element_size() * (co0 * ldw + ci0 * k * k)
     return ConvSeg(src.data_ptr(), wp, src.shape[1], c0, ci1 - ci0, cout0, co1 - co0, k, dil, ldw)
 
 
@@ -117,21 +166,65 @@ def conv_wgrad(ddst: torch.Tensor, s: ConvSeg, dw_ptr: int, accumulate=False, sp
                                      _st(ddst)), "csnet_train_conv_wgrad")
 
 
+_DT = {torch.float32: 0, torch.bfloat16: 2}        # CSNET_F32, CSNET_BF16
+
+
+def conv_plan_bf16(form: int, N: int, H: int, W: int, segs: Sequence[ConvSeg], splits_: int = 0):
+    """(splits, chain, workspace bytes) of a tensor-core (bf16) conv call."""
+    arr = (ConvSeg * len(segs))(*segs)
+    s, ch, ws = C.c_int32(), C.c_int32(), C.c_int64()
+    _ck(lib().csnet_train_conv_plan_bf16(form, N, H, W, arr, len(segs), splits_, C.byref(s), C.byref(ch), C.byref(ws)),
+        "csnet_train_conv_plan_bf16")
+    return s.value, ch.value, ws.value
+
+
+def _ws_bf16(form, N, H, W, segs, splits_, dev):
+    _, _, nb = conv_plan_bf16(form, N, H, W, segs, splits_)
+    return torch.empty(max(nb // 4, 1), dtype=torch.float32, device=dev), nb
+
+
+def conv_fwd_bf16(dst: torch.Tensor, segs: Sequence[ConvSeg], bias: Optional[int] = None, accumulate=False, splits_=0):
+    """conv_fwd on bf16 sources and weights (tensor cores); dst bf16 or fp32."""
+    N, Cd, H, W = dst.shape
+    ws, nb = _ws_bf16(0, N, H, W, segs, splits_, dst.device)
+    arr = (ConvSeg * len(segs))(*segs)
+    _ck(lib().csnet_train_conv_fwd_bf16(dst.data_ptr(), _DT[dst.dtype], N, Cd, H, W, arr, len(segs), bias, int(accumulate), splits_,
+                                        ws.data_ptr(), nb, _st(dst)), "csnet_train_conv_fwd_bf16")
+
+
+def conv_dgrad_bf16(dsrc: torch.Tensor, c0: int, cin: int, segs: Sequence[ConvSeg], accumulate=False, splits_=0):
+    N, Cs, H, W = dsrc.shape
+    ws, nb = _ws_bf16(1, N, H, W, segs, splits_, dsrc.device)
+    arr = (ConvSeg * len(segs))(*segs)
+    _ck(lib().csnet_train_conv_dgrad_bf16(dsrc.data_ptr(), _DT[dsrc.dtype], N, Cs, H, W, c0, cin, arr, len(segs), int(accumulate), splits_,
+                                          ws.data_ptr(), nb, _st(dsrc)), "csnet_train_conv_dgrad_bf16")
+
+
+def conv_wgrad_bf16(ddst: torch.Tensor, s: ConvSeg, dw_ptr: int, accumulate=False, splits_=0):
+    N, Cd, H, W = ddst.shape
+    ws, nb = _ws_bf16(2, N, H, W, [s], splits_, ddst.device)
+    _ck(lib().csnet_train_conv_wgrad_bf16(ddst.data_ptr(), N, Cd, H, W, C.byref(s), dw_ptr, int(accumulate), splits_, ws.data_ptr(), nb,
+                                          _st(ddst)), "csnet_train_conv_wgrad_bf16")
+
+
 def resize_fwd(src: torch.Tensor, size, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """F.interpolate(src, size, mode='bilinear', align_corners=False); with `out`, added to it in place."""
     N, Cs, Hs, Ws = src.shape
     acc = out is not None
     if out is None:
-        out = torch.empty((N, Cs, int(size[0]), int(size[1])), dtype=torch.float32, device=src.device)
-    _ck(lib().csnet_train_resize_fwd(src.data_ptr(), N, Cs, Hs, Ws, out.data_ptr(), out.shape[2], out.shape[3], int(acc), _st(src)),
-        "csnet_train_resize_fwd")
+        out = torch.empty((N, Cs, int(size[0]), int(size[1])), dtype=src.dtype, device=src.device)
+    if out.dtype != src.dtype:
+        raise runtime.EngineError(f"resize: {src.dtype} source, {out.dtype} destination")
+    fn = lib().csnet_train_resize_fwd_bf16 if src.dtype == torch.bfloat16 else lib().csnet_train_resize_fwd
+    _ck(fn(src.data_ptr(), N, Cs, Hs, Ws, out.data_ptr(), out.shape[2], out.shape[3], int(acc), _st(src)), "csnet_train_resize_fwd")
     return out
 
 
 def resize_bwd(ddst: torch.Tensor, src_hw) -> torch.Tensor:
     N, Cd, Hd, Wd = ddst.shape
-    d = torch.empty((N, Cd, int(src_hw[0]), int(src_hw[1])), dtype=torch.float32, device=ddst.device)
-    _ck(lib().csnet_train_resize_bwd(ddst.data_ptr(), N, Cd, Hd, Wd, d.data_ptr(), d.shape[2], d.shape[3], _st(ddst)), "csnet_train_resize_bwd")
+    d = torch.empty((N, Cd, int(src_hw[0]), int(src_hw[1])), dtype=ddst.dtype, device=ddst.device)
+    fn = lib().csnet_train_resize_bwd_bf16 if ddst.dtype == torch.bfloat16 else lib().csnet_train_resize_bwd
+    _ck(fn(ddst.data_ptr(), N, Cd, Hd, Wd, d.data_ptr(), d.shape[2], d.shape[3], _st(ddst)), "csnet_train_resize_bwd")
     return d
 
 
@@ -153,6 +246,7 @@ class Out(NamedTuple):
     W: int
     paths: tuple
     bias: Optional[int] = None   # index of a bias [C] added once
+    f32: bool = False            # with bf16 storage, an fp32 destination (cls_layer's 1-channel map)
 
 
 class ConvFn(torch.autograd.Function):
@@ -162,6 +256,9 @@ class ConvFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, outs, *tensors):
+        if _storage(tensors[outs[0].paths[0].src]) == torch.bfloat16:
+            return _conv_fwd_bf16(ctx, outs, tensors)
+        ctx.bf16 = False
         tensors = [_f32(t.detach()) for t in tensors]
         n = tensors[outs[0].paths[0].src].shape[0]
         dev = tensors[0].device
@@ -182,6 +279,8 @@ class ConvFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *douts):
+        if ctx.bf16:
+            return _conv_bwd_bf16(ctx, douts)
         outs = ctx.outs
         t = ctx.saved_tensors
         dev = t[0].device
@@ -224,12 +323,94 @@ class ConvFn(torch.autograd.Function):
         return (None, *grads)
 
 
+def _weights(outs) -> set:
+    return {p.w for o in outs for p in o.paths}
+
+
+def _conv_fwd_bf16(ctx, outs, tensors):
+    """ConvFn.forward with bf16 storage: activations bf16, each weight rounded once to bf16 (kept for the data gradient), bias fp32."""
+    wi, bi = _weights(outs), {o.bias for o in outs if o.bias is not None}
+    t = [cast_bf16(v.detach()) if i in wi else (_f32(v.detach()) if i in bi else _act(v.detach(), torch.bfloat16))
+         for i, v in enumerate(tensors)]
+    n = t[outs[0].paths[0].src].shape[0]
+    dev = t[0].device
+    res = []
+    for o in outs:
+        dst = torch.empty((n, o.C, o.H, o.W), dtype=torch.float32 if o.f32 else torch.bfloat16, device=dev)
+        slices = {}
+        for p in o.paths:
+            slices.setdefault(p.cout0, []).append(p)
+        for c0, ps in slices.items():
+            segs = [seg(t[p.src], t[p.w], p.co0, p.co1, p.ci0, p.ci1, cout0=p.cout0, dil=p.dil) for p in ps]
+            b = t[o.bias].data_ptr() + 4 * c0 if o.bias is not None else None
+            conv_fwd_bf16(dst, segs, bias=b)
+        res.append(dst)
+    ctx.bf16 = True
+    ctx.outs = outs
+    ctx.wshape = {i: tuple(tensors[i].shape) for i in wi}
+    ctx.save_for_backward(*t)
+    return tuple(res)
+
+
+def _conv_bwd_bf16(ctx, douts):
+    """ConvFn.backward with bf16 storage: data gradients bf16 on the rounded weights, weight gradients fp32.  An fp32 output gradient
+    (cls_layer's map) is rounded to bf16 for the GEMMs; the bias gradient reduces it in fp32."""
+    outs = ctx.outs
+    t = ctx.saved_tensors
+    dev = t[0].device
+    n = t[outs[0].paths[0].src].shape[0]
+    raw = list(douts)
+    dq = []
+    for k, o in enumerate(outs):
+        d = raw[k]
+        if d is None:
+            d = torch.zeros((n, o.C, o.H, o.W), dtype=torch.bfloat16, device=dev)
+        elif o.f32:
+            d = cast_bf16(d)
+        else:
+            d = _act(d, torch.bfloat16)
+        dq.append(d)
+    grads: List[Optional[torch.Tensor]] = [None] * len(t)
+    by_src = {}
+    for k, o in enumerate(outs):
+        for p in o.paths:
+            by_src.setdefault(p.src, []).append((k, p))
+    for s, kps in by_src.items():
+        if not ctx.needs_input_grad[1 + s]:
+            continue
+        x = t[s]
+        d = torch.empty_like(x)
+        segs = [seg(dq[k], t[p.w], p.co0, p.co1, p.ci0, p.ci1, cout0=p.cout0, dil=p.dil) for k, p in kps]
+        for i in range(0, len(segs), 8):                        # up to 8 K segments per call
+            conv_dgrad_bf16(d, 0, x.shape[1], segs[i:i + 8], accumulate=i > 0)
+        grads[s] = d
+    seen = {}
+    for k, o in enumerate(outs):
+        for p in o.paths:
+            if not ctx.needs_input_grad[1 + p.w]:
+                continue
+            if grads[p.w] is None:
+                grads[p.w] = torch.zeros(ctx.wshape[p.w], dtype=torch.float32, device=dev)
+            key = (p.w, p.co0, p.ci0)
+            s_ = seg(t[p.src], grads[p.w], p.co0, p.co1, p.ci0, p.ci1, cout0=p.cout0, dil=p.dil)
+            conv_wgrad_bf16(dq[k], s_, s_.w, accumulate=key in seen)
+            seen[key] = True
+        if o.bias is not None and ctx.needs_input_grad[1 + o.bias]:
+            if not o.f32 or raw[k] is None:
+                raise runtime.EngineError("bf16 storage: a bias gradient is reduced from an fp32 output gradient only")
+            dd = _f32(raw[k])
+            db = torch.empty(o.C, dtype=torch.float32, device=dev)
+            _ck(lib().csnet_train_bias_grad(dd.data_ptr(), n, o.C, o.H * o.W, 0, o.C, db.data_ptr(), _st(dd)), "csnet_train_bias_grad")
+            grads[o.bias] = db if grads[o.bias] is None else grads[o.bias] + db
+    return (None, *grads)
+
+
 class ResizeFn(torch.autograd.Function):
     """F.interpolate(src, size, mode='bilinear', align_corners=False), or `base + that` written into `base` (resize-add)."""
 
     @staticmethod
     def forward(ctx, src, size, base=None):
-        src = _f32(src.detach())
+        src = _act(src.detach(), _storage(src))
         ctx.src_hw = tuple(src.shape[2:])
         if base is not None:
             if not base.is_contiguous():
@@ -240,7 +421,7 @@ class ResizeFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dout):
-        dout = _f32(dout)
+        dout = _act(dout, _storage(dout))
         dsrc = resize_bwd(dout, ctx.src_hw) if ctx.needs_input_grad[0] else None
         has_base = len(ctx.needs_input_grad) > 2 and ctx.needs_input_grad[2]
         return dsrc, None, dout if has_base else None
@@ -251,14 +432,17 @@ class GnPreluFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, z, gamma, beta, slope):
-        z = _f32(z.detach())
+        z = _act(z.detach(), _storage(z))
         g, b, a = (_f32(v.detach()) for v in (gamma, beta, slope))
         n, c, h, w = z.shape
         mean = torch.empty(n * GN_GROUPS, dtype=torch.float32, device=z.device)
         var = torch.empty_like(mean)
         y = torch.empty_like(z)
-        _ck(lib().csnet_train_gn_stats(z.data_ptr(), n, c, h * w, GN_GROUPS, mean.data_ptr(), var.data_ptr(), _st(z)), "csnet_train_gn_stats")
-        _ck(lib().csnet_train_gn_prelu_fwd(z.data_ptr(), y.data_ptr(), n, c, h * w, GN_GROUPS, mean.data_ptr(), var.data_ptr(), g.data_ptr(),
+        bf = z.dtype == torch.bfloat16
+        stats = lib().csnet_train_gn_stats_bf16 if bf else lib().csnet_train_gn_stats
+        fwd = lib().csnet_train_gn_prelu_fwd_bf16 if bf else lib().csnet_train_gn_prelu_fwd
+        _ck(stats(z.data_ptr(), n, c, h * w, GN_GROUPS, mean.data_ptr(), var.data_ptr(), _st(z)), "csnet_train_gn_stats")
+        _ck(fwd(z.data_ptr(), y.data_ptr(), n, c, h * w, GN_GROUPS, mean.data_ptr(), var.data_ptr(), g.data_ptr(),
                                            b.data_ptr(), a.data_ptr(), GN_EPS, _st(z)), "csnet_train_gn_prelu_fwd")
         ctx.save_for_backward(z, mean, var, g, b, a)
         return y
@@ -266,12 +450,13 @@ class GnPreluFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         z, mean, var, g, b, a = ctx.saved_tensors
-        dy = _f32(dy)
+        dy = _act(dy, z.dtype)
         n, c, h, w = z.shape
         dz = torch.empty_like(z)
         dg, db, da = (torch.empty(c, dtype=torch.float32, device=z.device) for _ in range(3))
         ws = torch.empty(3 * n * c, dtype=torch.float32, device=z.device)
-        _ck(lib().csnet_train_gn_prelu_bwd(z.data_ptr(), dy.data_ptr(), dz.data_ptr(), n, c, h * w, GN_GROUPS, mean.data_ptr(), var.data_ptr(),
+        bwd = lib().csnet_train_gn_prelu_bwd_bf16 if z.dtype == torch.bfloat16 else lib().csnet_train_gn_prelu_bwd
+        _ck(bwd(z.data_ptr(), dy.data_ptr(), dz.data_ptr(), n, c, h * w, GN_GROUPS, mean.data_ptr(), var.data_ptr(),
                                            g.data_ptr(), b.data_ptr(), a.data_ptr(), GN_EPS, dg.data_ptr(), db.data_ptr(), da.data_ptr(),
                                            ws.data_ptr(), _st(z)), "csnet_train_gn_prelu_bwd")
         return dz, dg, db, da
@@ -333,7 +518,8 @@ def msblock(x, block) -> torch.Tensor:
 
 
 def csf_head(net, feats: Sequence[torch.Tensor], size) -> torch.Tensor:
-    """CSFNet.forward after the backbone (csf_res2net.py:253-258) on `net`'s parameters: logits [N, 1, H, W] at `size`."""
+    """CSFNet.forward after the backbone (csf_res2net.py:253-258) on `net`'s parameters: fp32 logits [N, 1, H, W] at `size`.  The
+    features' dtype (fp32, or bf16 with bf16 storage) is the head's activation storage; cls_layer writes its map in fp32."""
     fuse = net.fuse
     y = goct_conv_1x1(feats, fuse.conv.weights, fuse.alpha_in, fuse.alpha_out)
     y = [gn_prelu(t, fuse.bns[j], fuse.prelus[j]) if t is not None else None for j, t in enumerate(y)]
@@ -343,5 +529,5 @@ def csf_head(net, feats: Sequence[torch.Tensor], size) -> torch.Tensor:
     f0 = gn_prelu(f[0], f1.bns[0], f1.prelus[0])
     cl = net.cls_layer
     (out,) = ConvFn.apply((Out(cl.weight.shape[0], f0.shape[2], f0.shape[3], (Path(0, 1, 0, cl.weight.shape[0], 0, cl.weight.shape[1]),),
-                               bias=2),), f0, cl.weight, cl.bias)
+                               bias=2, f32=True),), f0, cl.weight, cl.bias)
     return ResizeFn.apply(out, tuple(size))

@@ -9,7 +9,8 @@ Split of the forward:
   * CSF head (`fuse` -> `ms` -> `fuse1x1` -> `cls_layer` -> bilinear to the input size): parameter containers lowered by compiler_r.py to one
     fused-op program on libcsnet_b200.so (GroupNorm variant).  No torch fallback for the head.
   * Training: when autograd records, the backbone runs on torch autograd and the head on modular_r.py's autograd Functions over the
-    fp32 training kernels (csnet_train_conv_* / _gn_* / _resize_*), so solver.py's train loop runs unchanged.
+    training kernels (csnet_train_conv_* / _gn_* / _resize_*, or their _bf16 twins with `train_storage = "bf16"`), so solver.py's
+    train loop runs unchanged.
 """
 from __future__ import annotations
 
@@ -172,6 +173,7 @@ class CSFNet(nn.Module):
         self.fuse1x1 = gOctaveCBR(cout, cout, kernel_size=(1, 1), padding=0, alpha_in=compiler_r.FUSE_OUT_SPLIT, alpha_out=[1])
         self.cls_layer = nn.Conv2d(cout, num_classes, kernel_size=1)
         self.precision = "fp32"
+        self.train_storage = "fp32"              # training activation storage, "fp32" or "bf16" (CSFTrainer(storage=...), DESIGN §7.3)
         self._plans = OrderedDict()              # (h, w, precision, device) -> head plan, least recently used first
         self._plan_version = {}
         self.plan_budget = PLAN_BUDGET
@@ -211,10 +213,15 @@ class CSFNet(nn.Module):
         if not x.is_cuda:
             raise runtime.EngineError("CSFNet (CUDA engine) needs CUDA tensors; there is no CPU path")
         if torch.is_grad_enabled() and (x.requires_grad or any(q.requires_grad for q in self.parameters())):
-            # training (CSF+Res2Net/solver.py:train): the backbone on torch autograd (cuDNN, fp32), the head on our fp32 training kernels
-            # (modular_r), logits with a grad_fn at the input's size
+            # training (CSF+Res2Net/solver.py:train): the backbone on torch autograd (cuDNN), the head on our training kernels (modular_r),
+            # logits with a grad_fn at the input's size.  train_storage "bf16": the backbone under bf16 autocast, its bf16 features
+            # through the head's bf16 kernels; "fp32" (default): fp32 throughout.  set_precision does not apply to training.
             from .. import modular_r
 
+            if modular_r.train_dtype(self) == torch.bfloat16:
+                with torch.autocast("cuda", dtype=torch.bfloat16):
+                    feats = [f.to(torch.bfloat16).contiguous() for f in self.base(x.float())]
+                return modular_r.csf_head(self, feats, x.shape[2:])
             return modular_r.csf_head(self, self.base(x.float()), x.shape[2:])
         self._check_inference()
         feats = self.backbone(x.float())

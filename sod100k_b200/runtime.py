@@ -13,7 +13,7 @@ from . import ir
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libcsnet_b200.so")
-ABI_VERSION = 13
+ABI_VERSION = 14
 PARAM_EPOCH = 0      # bumped by in-place parameter updates that bypass torch's version counters (FusedAdam)
 _lib = None
 
@@ -30,7 +30,10 @@ SYMBOLS = ("csnet_abi_version", "csnet_last_error", "csnet_device_count", "csnet
            "csnet_csf_input_u8", "csnet_csf_maps_u8", "csnet_salmetric_csf_u8", "csnet_csf_train_batch_u8", "csnet_train_bce_sum",
            "csnet_train_bn_stats_bf16", "csnet_train_bn_prelu_fwd_bf16", "csnet_train_bn_prelu_bwd_bf16", "csnet_train_dw_conv_bf16",
            "csnet_train_dw_wgrad_bf16", "csnet_train_dw_bwd_bf16", "csnet_train_mix_fwd_bf16", "csnet_train_mix_dgrad_bf16",
-           "csnet_train_mix_wgrad_bf16", "csnet_train_pool_fwd_bf16", "csnet_train_pool_bwd_bf16")
+           "csnet_train_mix_wgrad_bf16", "csnet_train_pool_fwd_bf16", "csnet_train_pool_bwd_bf16", "csnet_train_cast_bf16",
+           "csnet_train_conv_plan_bf16", "csnet_train_conv_fwd_bf16", "csnet_train_conv_dgrad_bf16", "csnet_train_conv_wgrad_bf16",
+           "csnet_train_gn_stats_bf16", "csnet_train_gn_prelu_fwd_bf16", "csnet_train_gn_prelu_bwd_bf16", "csnet_train_resize_fwd_bf16",
+           "csnet_train_resize_bwd_bf16")
 
 
 class EngineError(RuntimeError):

@@ -159,7 +159,9 @@ class CSFTrainer:
     """CSF+Res2Net/solver.py:train's step on the device: forward on the module's training path in eval mode (frozen BatchNorm, as
     solver.py:49 keeps the net), BCE summed over the batch / (iter_size * batch_size) (BceSumFn, no host sync), backward into one flat
     gradient bucket (FlatGrads), and every iter_size-th micro-step one FusedAdam launch (torch.optim.Adam with L2 weight decay, betas
-    (0.9, 0.999), eps 1e-8) over the trainable parameters, then a zeroed bucket.  Training runs in fp32 whatever set_precision says.
+    (0.9, 0.999), eps 1e-8) over the trainable parameters, then a zeroed bucket.  `storage` sets net.train_storage: "fp32" (default)
+    or "bf16" (bf16 activations, the backbone under autocast, the head's convolutions on tensor cores; DESIGN.md §7.3).  set_precision
+    applies to inference only.
 
         trainer = CSFTrainer(net, iter_size=10)
         for epoch in range(epochs):
@@ -172,10 +174,13 @@ class CSFTrainer:
     Gradients live in the bucket: a net.zero_grad() (or anything else that replaces p.grad) makes the next step raise EngineError."""
 
     def __init__(self, net, lr: float = 5e-5, weight_decay: float = 5e-4, iter_size: int = 10, lr_decay_epochs=(15,),
-                 batch_size: int = 1):
+                 batch_size: int = 1, storage: str = "fp32"):
         if int(batch_size) < 1:
             raise ValueError(f"batch_size must be >= 1, got {batch_size}")
+        if storage not in T.STORAGES:
+            raise ValueError(f"storage must be one of {sorted(T.STORAGES)}, got {storage!r}")
         self.net = net
+        net.train_storage = storage
         self.schedule = CSFSchedule(iter_size, lr, lr_decay_epochs)
         self.divisor = self.schedule.iter_size * int(batch_size)
         self.weight_decay = float(weight_decay)
