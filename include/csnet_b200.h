@@ -423,6 +423,26 @@ int csnet_train_pool_fwd_bf16(const void* src, int32_t N, int32_t Cs, int32_t c0
 int csnet_train_pool_bwd_bf16(const void* dpool, const uint8_t* idx, int32_t N, int32_t cin, int32_t Hs, int32_t Ws, int32_t pre_avg,
                               int32_t pool, void* dsrc, void* stream);
 
+/* ---- synchronized BatchNorm + PReLU (nn.SyncBatchNorm over G ranks; csrc/bn_sync.cu) -------------------------------------------
+ * Each direction is two calls around one all-reduce(SUM) the caller issues on a zeroed float64 row buffer in which rank `rank`
+ * fills only its own row, so the sum is an exact gather and every rank merges the same rows in rank order.  z / dy / dz hold
+ * `dtype` (CSNET_F32 or CSNET_BF16); the forward between the two halves is csnet_train_bn_prelu_fwd[_bf16] with the merged
+ * statistics.  No floating-point atomics: the same bits on every run. */
+/* row `rank` of rows [G][C][3] = (count, mean, M2 = sum (z - mean)^2) of each channel over this rank's z [N][C][HW] */
+int csnet_train_bn_sync_partial(const void* z, int32_t dtype, int32_t N, int32_t C, int32_t HW, int32_t rank, double* rows,
+                                void* stream);
+/* rows 0..G-1 merged in rank order (Chan's pairwise update, float64): mean / biased var [C] of the global batch; count[0]: its size */
+int csnet_train_bn_sync_merge(const double* rows, int32_t G, int32_t C, float* mean, float* var, double* count, void* stream);
+/* mean / var: the merged statistics.  dgamma / dbeta / dslope [C]: this rank's parameter gradients; row `rank` of rows [G][C][2] =
+ * (sum du, sum du * xhat) over this rank's batch */
+int csnet_train_bn_sync_bwd_reduce(const void* z, const void* dy, int32_t dtype, int32_t N, int32_t C, int32_t HW, const float* mean,
+                                   const float* var, const float* gamma, const float* beta, const float* slope, float eps, float* dgamma,
+                                   float* dbeta, float* dslope, int32_t rank, double* rows, void* stream);
+/* dz = gamma r (du - S1 / M - xhat S2 / M), S1 / S2 the rows of all G ranks summed in rank order, M = count[0] (global) */
+int csnet_train_bn_sync_bwd_apply(const void* z, const void* dy, void* dz, int32_t dtype, int32_t N, int32_t C, int32_t HW, const float* mean,
+                                  const float* var, const float* gamma, const float* beta, const float* slope, float eps, const double* rows,
+                                  int32_t G, const double* count, void* stream);
+
 /* ---- CSF+Res2Net head training (fp32; sod100k_b200/modular_r.py wraps them) ---------------------------------------------------
  * Convolutions as an fp32 FMA implicit GEMM (csrc/gemm_f32.cuh).  One segment is one stride-1 convolution of a channel slice of
  * `src` with a weight slice: element (co, ci, ky, kx) of the weight is w[co * ldw + ci * ksize * ksize + ky * ksize + kx]

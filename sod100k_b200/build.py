@@ -8,7 +8,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libcsnet_b200.so")
-SOURCES = ["plan.cu", "train_ops.cu", "train_csf.cu", "train_bf16.cu", "train_csf_bf16.cu"]
+SOURCES = ["plan.cu", "train_ops.cu", "train_csf.cu", "train_bf16.cu", "train_csf_bf16.cu", "bn_sync.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-O3,-Wall", "-shared", "-cudart", "shared"]
 

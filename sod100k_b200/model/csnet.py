@@ -288,7 +288,7 @@ class CSNet(nn.Module):
         for m in self.modules():
             if isinstance(m, gOctaveCBR):
                 for n in m.modules():
-                    if isinstance(n, nn.BatchNorm2d) and n.weight.grad is not None:
+                    if isinstance(n, (nn.BatchNorm2d, nn.SyncBatchNorm)) and n.weight.grad is not None:
                         n.weight.grad.data.add_(s * torch.sign(n.weight.data))
 
 

@@ -55,7 +55,7 @@ def _goct_conv(m, in_shapes):
 
 def _norm_act(bn, prelu, shape):
     n = shape[0] * shape[1] * shape[2]
-    return (4 * n if isinstance(bn, nn.BatchNorm2d) else 0) + (3 * n if isinstance(prelu, nn.PReLU) else 0)
+    return (4 * n if isinstance(bn, (nn.BatchNorm2d, nn.SyncBatchNorm)) else 0) + (3 * n if isinstance(prelu, nn.PReLU) else 0)
 
 
 def print_model_parm_flops(model, inputsize, device=-1):

@@ -33,7 +33,8 @@ SYMBOLS = ("csnet_abi_version", "csnet_last_error", "csnet_device_count", "csnet
            "csnet_train_mix_wgrad_bf16", "csnet_train_pool_fwd_bf16", "csnet_train_pool_bwd_bf16", "csnet_train_cast_bf16",
            "csnet_train_conv_plan_bf16", "csnet_train_conv_fwd_bf16", "csnet_train_conv_dgrad_bf16", "csnet_train_conv_wgrad_bf16",
            "csnet_train_gn_stats_bf16", "csnet_train_gn_prelu_fwd_bf16", "csnet_train_gn_prelu_bwd_bf16", "csnet_train_resize_fwd_bf16",
-           "csnet_train_resize_bwd_bf16")
+           "csnet_train_resize_bwd_bf16", "csnet_train_bn_sync_partial", "csnet_train_bn_sync_merge", "csnet_train_bn_sync_bwd_reduce",
+           "csnet_train_bn_sync_bwd_apply")
 
 
 class EngineError(RuntimeError):

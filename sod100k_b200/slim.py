@@ -20,6 +20,8 @@ import torch.nn as nn
 
 from . import runtime
 
+# a model converted by nn.SyncBatchNorm.convert_sync_batchnorm keeps its BatchNorm names and state_dict keys: it slims the same
+_BN = (nn.BatchNorm2d, nn.SyncBatchNorm)
 
 def _gather(v: torch.Tensor, out_idx: torch.Tensor, in_idx, shape) -> torch.Tensor:
     """zeros(shape) with [len(out_idx), len(in_idx)] leading block = v[out_idx][:, in_idx] (in_idx None: all of dim 1 / a vector)."""
@@ -70,7 +72,7 @@ def finetune_config(model, base_layer_config, thres):
             continue
         layer = len(masks)
         this_out = [int(c) for c in np.asarray(base_layer_config[layer][1]).reshape(-1)]
-        gam = torch.cat([b.weight.detach().reshape(-1) for b in m.modules() if isinstance(b, nn.BatchNorm2d)])
+        gam = torch.cat([b.weight.detach().reshape(-1) for b in m.modules() if isinstance(b, _BN)])
         keep = gam.abs() >= thres                                   # reference: mask[abs(gamma) < thres] = 0
         parts = list(torch.split(keep, this_out)) if sum(this_out) == keep.numel() else None
         if parts is None:
@@ -131,7 +133,7 @@ def _load_goct_cbr(M, mod, full, this_mask, last_mask, new_sd):
         if isinstance(m, M.gOctaveConv):
             key = f"{full}.{name}.weight"
             new_sd[key] = _gather(m.weight, _idx(this_mask), _idx(last_mask), new_sd[key].shape)
-        elif isinstance(m, nn.BatchNorm2d):
+        elif isinstance(m, _BN):
             _load_bn(m, f"{full}.{name}", this_mask[int(name.split(".")[-1])], new_sd)
         elif isinstance(m, nn.PReLU):
             _load_prelu(m, f"{full}.{name}", this_mask[int(name.split(".")[-1])], new_sd)
@@ -144,7 +146,7 @@ def _load_dw_cbr(M, mod, full, this_mask, new_sd):
             key = f"{full}.{name}.weight"
             if key in new_sd:
                 new_sd[key] = _gather(m.weight, torch.nonzero(this_mask[int(name.split(".")[-1])]).reshape(-1), None, new_sd[key].shape)
-        elif isinstance(m, nn.BatchNorm2d):
+        elif isinstance(m, _BN):
             _load_bn(m, f"{full}.{name}", this_mask[int(name.split(".")[-1])], new_sd)
         elif isinstance(m, nn.PReLU):
             _load_prelu(m, f"{full}.{name}", this_mask[int(name.split(".")[-1])], new_sd)
@@ -166,7 +168,7 @@ def _load_pall_ms(M, mod, full, this_mask, last_mask, new_sd):
                 key = f"{full}.{name}.{cname}.weight"
                 if key in new_sd:
                     new_sd[key] = _gather(c.weight, torch.nonzero(sub).reshape(-1), in_idx, new_sd[key].shape)
-        elif isinstance(m, nn.BatchNorm2d):
+        elif isinstance(m, _BN):
             _load_bn(m, f"{full}.{name}", this_mask[int(name.split(".")[-2])], new_sd)
         elif isinstance(m, nn.PReLU):
             _load_prelu(m, f"{full}.{name}", this_mask[int(name.split(".")[-2])], new_sd)

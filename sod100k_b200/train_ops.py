@@ -59,6 +59,10 @@ def lib():
         l.csnet_train_mix_wgrad_bf16.argtypes = [vp, i32, i32, i32, i32, i32, C.POINTER(TrainPath), f32p, i32, vp]
         l.csnet_train_pool_fwd_bf16.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, vp, vp]
         l.csnet_train_pool_bwd_bf16.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, vp, vp]
+        l.csnet_train_bn_sync_partial.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp]
+        l.csnet_train_bn_sync_merge.argtypes = [vp, i32, i32, f32p, f32p, vp, vp]
+        l.csnet_train_bn_sync_bwd_reduce.argtypes = [vp, vp, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, f, f32p, f32p, f32p, i32, vp, vp]
+        l.csnet_train_bn_sync_bwd_apply.argtypes = [vp, vp, vp, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, f, vp, i32, vp, vp]
         _lib = l
     return _lib
 
@@ -319,18 +323,100 @@ class BnPreluFn(torch.autograd.Function):
         return dz, dgamma, dbeta, dslope, None, None
 
 
+class SyncBnPreluFn(torch.autograd.Function):
+    """BnPreluFn with the statistics of the batch spread over the ranks of `group` (nn.SyncBatchNorm): per direction, the
+    rank's partial sums go into its own row of a zeroed float64 buffer, one all_reduce(SUM) over the group gathers the rows
+    exactly, and every rank merges them in rank order (csnet_train_bn_sync_*).  Also returns the global mean / biased
+    variance, the global element count (a float64 device scalar) and the per-image channel means of this rank's output.
+    dgamma / dbeta / dslope are this rank's: the gradient all-reduce of the step sums them."""
+
+    @staticmethod
+    def forward(ctx, z, gamma, beta, slope, group, rank, world):
+        import torch.distributed as dist
+
+        z = _act(z)
+        code, sfx = _code(z.dtype), "_bf16" if z.dtype == torch.bfloat16 else ""
+        n, c, h, w = z.shape
+        st = _stream(z)
+        g, b, a = _f32(gamma.detach()), _f32(beta.detach()), _f32(slope.detach())
+        rows = torch.zeros((world, c, 3), dtype=torch.float64, device=z.device)
+        _ck(lib().csnet_train_bn_sync_partial(z.data_ptr(), code, n, c, h * w, rank, rows.data_ptr(), st), "csnet_train_bn_sync_partial")
+        dist.all_reduce(rows, op=dist.ReduceOp.SUM, group=group)
+        mean = torch.empty(c, dtype=torch.float32, device=z.device)
+        var = torch.empty_like(mean)
+        count = torch.empty(1, dtype=torch.float64, device=z.device)
+        _ck(lib().csnet_train_bn_sync_merge(rows.data_ptr(), world, c, mean.data_ptr(), var.data_ptr(), count.data_ptr(), st),
+            "csnet_train_bn_sync_merge")
+        y = torch.empty_like(z)
+        gap = torch.empty((n, c), dtype=torch.float32, device=z.device)
+        _ck(getattr(lib(), "csnet_train_bn_prelu_fwd" + sfx)(z.data_ptr(), y.data_ptr(), n, c, h * w, mean.data_ptr(), var.data_ptr(),
+                                                             g.data_ptr(), b.data_ptr(), a.data_ptr(), BN_EPS, gap.data_ptr(), st),
+            "csnet_train_bn_prelu_fwd" + sfx)
+        ctx.save_for_backward(z, mean, var, count, g, b, a)
+        ctx.group, ctx.rank, ctx.world = group, rank, world
+        ctx.mark_non_differentiable(mean, var, count, gap)
+        return y, mean, var, count, gap
+
+    @staticmethod
+    def backward(ctx, dy, _dm, _dv, _dc, _dg):
+        import torch.distributed as dist
+
+        z, mean, var, count, g, b, a = ctx.saved_tensors
+        dy = _act(dy) if z.dtype == torch.bfloat16 else _f32(dy)
+        code = _code(z.dtype)
+        n, c, h, w = z.shape
+        st = _stream(z)
+        dz = torch.empty_like(z)
+        dgamma, dbeta, dslope = (torch.empty(c, dtype=torch.float32, device=z.device) for _ in range(3))
+        rows = torch.zeros((ctx.world, c, 2), dtype=torch.float64, device=z.device)
+        _ck(lib().csnet_train_bn_sync_bwd_reduce(z.data_ptr(), dy.data_ptr(), code, n, c, h * w, mean.data_ptr(), var.data_ptr(), g.data_ptr(),
+                                                 b.data_ptr(), a.data_ptr(), BN_EPS, dgamma.data_ptr(), dbeta.data_ptr(), dslope.data_ptr(),
+                                                 ctx.rank, rows.data_ptr(), st), "csnet_train_bn_sync_bwd_reduce")
+        dist.all_reduce(rows, op=dist.ReduceOp.SUM, group=ctx.group)
+        _ck(lib().csnet_train_bn_sync_bwd_apply(z.data_ptr(), dy.data_ptr(), dz.data_ptr(), code, n, c, h * w, mean.data_ptr(), var.data_ptr(),
+                                                g.data_ptr(), b.data_ptr(), a.data_ptr(), BN_EPS, rows.data_ptr(), ctx.world, count.data_ptr(),
+                                                st), "csnet_train_bn_sync_bwd_apply")
+        return dz, dgamma, dbeta, dslope, None, None, None
+
+
+def sync_group(bn):
+    """The process group whose batch statistics `bn` normalises by, or None for the statistics of this process's batch: an
+    nn.SyncBatchNorm in training mode synchronizes over its process_group (None: the default group) when torch.distributed
+    is initialised and that group has more than one rank."""
+    if not (isinstance(bn, torch.nn.SyncBatchNorm) and bn.training):
+        return None
+    import torch.distributed as dist
+
+    if not (dist.is_available() and dist.is_initialized()):
+        return None
+    group = bn.process_group if bn.process_group is not None else dist.group.WORLD
+    return group if dist.get_world_size(group) > 1 else None
+
+
 def bn_prelu_train(z, bn: torch.nn.BatchNorm2d, prelu: torch.nn.PReLU):
-    """Apply + update running statistics the way nn.BatchNorm2d does in train mode (momentum 0.1, unbiased variance)."""
+    """Apply + update running statistics the way nn.BatchNorm2d does in train mode (momentum 0.1, unbiased variance); an
+    nn.SyncBatchNorm takes the statistics of its process group's whole batch (sync_group)."""
     if not bn.training:                                  # frozen statistics (module left in eval mode)
         y, _, _, gap = BnPreluFn.apply(z, bn.weight, bn.bias, prelu.weight, bn.running_mean, bn.running_var)
         return y, gap
-    y, mean, var, gap = BnPreluFn.apply(z, bn.weight, bn.bias, prelu.weight)
+    group = sync_group(bn)
+    if group is None:
+        y, mean, var, gap = BnPreluFn.apply(z, bn.weight, bn.bias, prelu.weight)
+        m = z.shape[0] * z.shape[2] * z.shape[3]
+        unbias = m / max(m - 1, 1)
+    else:
+        import torch.distributed as dist
+
+        # a checkpointed re-run issues the same collective in the same backward order on every rank, and gets the same bits
+        y, mean, var, count, gap = SyncBnPreluFn.apply(z, bn.weight, bn.bias, prelu.weight, group, dist.get_rank(group),
+                                                       dist.get_world_size(group))
     if bn.track_running_stats and not RECOMPUTING:
         with torch.no_grad():
-            m = z.shape[0] * z.shape[2] * z.shape[3]
+            if group is not None:
+                unbias = (count / (count - 1).clamp_min(1)).float()
             mom = 0.1 if bn.momentum is None else bn.momentum
             bn.running_mean.mul_(1 - mom).add_(mean, alpha=mom)
-            bn.running_var.mul_(1 - mom).add_(var * (m / max(m - 1, 1)), alpha=mom)
+            bn.running_var.mul_(1 - mom).add_(var * unbias, alpha=mom)
             bn.num_batches_tracked += 1
     return y, gap
 

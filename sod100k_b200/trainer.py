@@ -2,9 +2,13 @@
 train-mode forward -> mean BCE-with-logits (+ WEIGHT * get_flops()) -> backward -> [DP: one all-reduce of the single
 flat gradient bucket] -> Adam in the reference's two weight-decay groups (train.py:97-123).
 
-Data parallelism (SURVEY.md §8e): one process per GPU, local BatchNorm statistics (the reference has no SyncBN), the
-only collective is the all-reduce(sum)/world of ONE flat fp32 bucket holding every gradient (140 894 floats for
-csnet-L-x2) — every `p.grad` is a view into that bucket, so there is no flatten / unflatten copy.
+Data parallelism (SURVEY.md §8e): one process per GPU; the gradients travel in the all-reduce(sum)/world of ONE flat fp32
+bucket holding every gradient (140 894 floats for csnet-L-x2) — every `p.grad` is a view into that bucket, so there is no
+flatten / unflatten copy.  BatchNorm statistics are each rank's own unless the model was converted with
+`nn.SyncBatchNorm.convert_sync_batchnorm(model, group)`: then every train-mode BatchNorm normalises by the statistics of the
+group's whole batch, with one small float64 all-reduce per BatchNorm call in each direction (train_ops.SyncBnPreluFn, DESIGN
+§5.1), so a G-GPU step at global batch B computes the step one GPU computes at batch B.  The dynamic-weight-decay term stays per
+rank (each rank's own activations); the bucket's mean averages it.
 """
 from __future__ import annotations
 
